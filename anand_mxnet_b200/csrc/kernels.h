@@ -202,6 +202,28 @@ void LaunchMultiTensorFinalize(const MTTensor* tensors, int n_tensors, const flo
 void LaunchMultiLars(int n, float* out, const float* lrs, const float* wsq, const float* gsq,
                      const float* wds, float eta, float eps, float rescale, cudaStream_t stream);
 
+// ---- single-tensor optimizer operators of the callback route (update_kernels.cu) ----
+// nag_mom_update, mp_nag_mom_update, signsgd_update, signum_update, rmsprop_update,
+// rmspropalex_update, ftml_update, ftrl_update (optimizer_op-inl.h:1061-1222, 1953-2158, 2344-2431)
+enum UpdOp : int { kUpdNAG = 0, kUpdMPNAG, kUpdSignSGD, kUpdSignum, kUpdRMSProp, kUpdRMSPropAlex,
+                   kUpdFTML, kUpdFtrl };
+struct UpdateLaunch {
+  int op = kUpdNAG;
+  int dtype = 0;                 // of w / g / out: kFloat32, or kFloat16 / kBfloat16 for kUpdMPNAG
+  const void* w = nullptr;       // weight (read; may be the same storage as out)
+  const void* g = nullptr;
+  void* out = nullptr;
+  float* s[3] = {nullptr, nullptr, nullptr};  // fp32 states in the operator's input order
+                                              // (mp_nag: mom, weight32)
+  size_t n = 0;
+  bool out_is_w = false;  // nag_mom_update reads the weight again after storing out
+  // hyper-parameters, by value (FTML: p1 = powf(beta1, t), p2 = powf(beta2, t) from the host)
+  float lr = 0.f, wd = 0.f, rescale = 1.f, clip = -1.f, momentum = 0.f, wd_lh = 0.f, gamma1 = 0.f,
+        gamma2 = 0.f, eps = 0.f, clip_weights = -1.f, beta1 = 0.f, beta2 = 0.f, p1 = 0.f, p2 = 0.f,
+        lamda1 = 0.f, beta = 0.f;
+};
+void LaunchUpdateOp(const UpdateLaunch& L, cudaStream_t stream);
+
 // ---- 2-bit gradient compression with residual (compress_kernels.cu;
 // src/kvstore/gradient_compression-inl.h:40-132, comm.h:552-596 ReduceCompressed) ----
 // residual += grad; >= +t -> code 11, residual -= t; <= -t -> code 10, residual += t; else 00.

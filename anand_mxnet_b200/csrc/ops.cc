@@ -16,6 +16,9 @@ namespace b200kv {
 
 void PlanChunks(uint64_t goff, size_t size, uint32_t key_slot, int ndev, int owner_fixed,
                 std::vector<std::vector<ChunkDesc>>* per_slot);  // kvstore.cc
+// NAG / Signum / RMSProp / FTML / Ftrl operators; false when `name` is not one of them
+bool UpdateOp(const std::string& name, const std::vector<NDArray>& in, std::vector<NDArray>* outputs,
+              const Params& p);  // update_ops.cc
 
 namespace {
 
@@ -32,7 +35,10 @@ const std::map<std::string, OpInfo>& Registry() {
           "preloaded_multi_mp_sgd_update", "preloaded_multi_mp_sgd_mom_update", "_adamw_update",
           "_mp_adamw_update", "_multi_adamw_update", "_multi_mp_adamw_update", "lamb_update_phase1",
           "lamb_update_phase2", "mp_lamb_update_phase1", "mp_lamb_update_phase2",
-          "_multi_lamb_update", "_multi_mp_lamb_update"}) {
+          "_multi_lamb_update", "_multi_mp_lamb_update",
+          // single-tensor operators of the callback route (update_ops.cc)
+          "nag_mom_update", "mp_nag_mom_update", "signsgd_update", "signum_update", "rmsprop_update",
+          "rmspropalex_update", "ftml_update", "ftrl_update"}) {
       r[n] = OpInfo{n};
     }
   }
@@ -341,6 +347,7 @@ void InvokeOp(const OpInfo* op, const std::vector<NDArray>& in, std::vector<NDAr
     return;
   }
   if (MultiTensorOp(n, in, outputs, p)) return;  // multi_ops.cc: sum_sq, lars, adamw, lamb
+  if (UpdateOp(n, in, outputs, p)) return;       // update_ops.cc: nag, signum, rmsprop, ftml, ftrl
   if (n.rfind("multi_", 0) == 0 || n.rfind("preloaded_multi_", 0) == 0) {
     // multi_[mp_]sgd[_mom]_update (optimizer_op-inl.h:207-380) and the preloaded_ forms
     // (contrib/preloaded_multi_sgd-inl.h:154-330: same kernel, lrs / wds are two trailing INPUT

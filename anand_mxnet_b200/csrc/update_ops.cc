@@ -1,0 +1,257 @@
+// update_ops.cc -- host side of the single-tensor optimizer operators that the reference's NAG,
+// Signum, RMSProp, FTML and Ftrl optimizers call from their `update` (the per-key updater callback
+// of the store, and the local updaters of update_on_kvstore=False). Kernels: update_kernels.cu.
+//
+// Reference operator definitions (inputs, parameter structs, kernels):
+//   nag_mom_update, mp_nag_mom_update    src/operator/optimizer_op.cc:712-762, optimizer_op-inl.h:1032-1160
+//   ftml_update                          optimizer_op.cc:626-660, optimizer_op-inl.h:1163-1249
+//   rmsprop_update, rmspropalex_update   optimizer_op.cc:763-853, optimizer_op-inl.h:1915-2099
+//   ftrl_update                          optimizer_op.cc:854-890, optimizer_op-inl.h:2101-2183
+//   signsgd_update, signum_update        optimizer_op.cc:49-104, optimizer_op-inl.h:2319-2452
+//
+// Dense float32 arrays only (mp_nag_mom_update: float16 / bfloat16 weights with float32 mom and
+// weight32). The reference would densify a row_sparse gradient and run 16-bit weights of the other
+// operators in half precision; both are refused here before anything is launched.
+#include <cctype>
+#include <cerrno>
+#include <cmath>
+#include <limits>
+
+#include "kernels.h"
+#include "op_params.h"
+#include "ops.h"
+
+namespace b200kv {
+namespace {
+
+struct Spec {
+  const char* name;
+  int op;
+  int nin;                 // weight, grad, states...
+  const char* launch_name; // CountLaunch keeps the pointer
+  int bytes_per_elem;      // algorithmic traffic of one element (float32 / mp float16)
+};
+
+const Spec kSpecs[] = {
+    {"nag_mom_update", kUpdNAG, 3, "update_op(nag_mom_update)", 20},
+    {"mp_nag_mom_update", kUpdMPNAG, 4, "update_op(mp_nag_mom_update)", 20},
+    {"signsgd_update", kUpdSignSGD, 2, "update_op(signsgd_update)", 12},
+    {"signum_update", kUpdSignum, 3, "update_op(signum_update)", 20},
+    {"rmsprop_update", kUpdRMSProp, 3, "update_op(rmsprop_update)", 20},
+    {"rmspropalex_update", kUpdRMSPropAlex, 5, "update_op(rmspropalex_update)", 36},
+    {"ftml_update", kUpdFTML, 5, "update_op(ftml_update)", 36},
+    {"ftrl_update", kUpdFtrl, 4, "update_op(ftrl_update)", 28},
+};
+
+// Restatement of dmlc::stod == ParseFloat<double, true> (3rdparty/dmlc-core/include/dmlc/
+// strtonum.h:99-254, 497-510), the parser of double fields (FieldEntry<double>, parameter.h:1106-1125)
+// such as FTML's epsilon. Like stof it is not correctly rounded: float(int part) + double(frac
+// digits) / double(10^k), then scaled by powers of ten.
+double DmlcStod(const std::string& s) {
+  constexpr unsigned kMaxExponent = 308U;
+  constexpr double kMaxSigForMaxExp = 1.79769313486231570;
+  constexpr double kMaxSigForNegMaxExp = 2.22507385850720139;
+  constexpr int kStrtofMaxDigits = 19;
+  const char* p = s.c_str();
+  while (std::isspace(static_cast<unsigned char>(*p))) ++p;
+  bool positive = true;
+  if (*p == '-') {
+    positive = false;
+    ++p;
+  } else if (*p == '+') {
+    ++p;
+  }
+  auto finish = [&](double value, const char* end) -> double {
+    KV_CHECK(end != s.c_str() && *end == '\0')
+        << "Invalid Parameter format: expect double but value='" << s << "'";
+    return value;
+  };
+  {
+    int i = 0;
+    while (i < 8 && static_cast<char>((*p) | 32) == "infinity"[i]) { ++i; ++p; }
+    if (i == 3 || i == 8) {
+      return finish(positive ? std::numeric_limits<double>::infinity()
+                             : -std::numeric_limits<double>::infinity(), p);
+    }
+    p -= i;
+    i = 0;
+    while (i < 3 && static_cast<char>((*p) | 32) == "nan"[i]) { ++i; ++p; }
+    if (i == 3) return finish(std::numeric_limits<double>::quiet_NaN(), p);
+    p -= i;
+  }
+  const char* num_start = p;
+  uint64_t predec = 0;
+  for (; std::isdigit(static_cast<unsigned char>(*p)); ++p) {
+    predec = predec * 10ULL + static_cast<uint64_t>(*p - '0');
+  }
+  double value = static_cast<double>(predec);
+  if (*p == '.') {
+    uint64_t pow10 = 1, val2 = 0;
+    int digit_cnt = 0;
+    ++p;
+    while (std::isdigit(static_cast<unsigned char>(*p))) {
+      if (digit_cnt < kStrtofMaxDigits) {
+        val2 = val2 * 10ULL + static_cast<uint64_t>(*p - '0');
+        pow10 *= 10ULL;
+      }
+      ++p;
+      ++digit_cnt;
+    }
+    value += static_cast<double>(val2) / static_cast<double>(pow10);
+  }
+  KV_CHECK(p != num_start) << "Invalid Parameter format: expect double but value='" << s << "'";
+  if (*p == 'e' || *p == 'E') {
+    ++p;
+    bool frac = false;
+    double scale = 1.0;
+    unsigned expon = 0;
+    if (*p == '-') {
+      frac = true;
+      ++p;
+    } else if (*p == '+') {
+      ++p;
+    }
+    for (; std::isdigit(static_cast<unsigned char>(*p)); ++p) {
+      expon = expon * 10U + static_cast<unsigned>(*p - '0');
+    }
+    KV_CHECK(expon <= kMaxExponent) << "Out of range value '" << s << "'";
+    KV_CHECK(!(expon == kMaxExponent && ((!frac && value > kMaxSigForMaxExp) ||
+                                         (frac && value < kMaxSigForNegMaxExp))))
+        << "Out of range value '" << s << "'";
+    while (expon >= 8U) { scale *= static_cast<double>(1E8f); expon -= 8U; }
+    while (expon > 0U) { scale *= static_cast<double>(10.0f); expon -= 1U; }
+    value = frac ? (value / scale) : (value * scale);
+  }
+  if (*p == 'f' || *p == 'F') ++p;
+  return finish(positive ? value : -value, p);
+}
+
+float Required(const Params& p, const char* key, const std::string& op) {
+  KV_CHECK(Find(p, key) != nullptr) << "Required parameter " << key << " of " << op << " is missing";
+  return GetF(p, key, 0.f);
+}
+
+// dmlc::Parameter set_range(lo, hi) (parameter.h:752-762)
+float InRange(float v, const char* key, float lo, float hi) {
+  KV_CHECK(!(v < lo || v > hi)) << "value " << v << " for Parameter " << key << " exceed bound [" << lo
+                                << ',' << hi << ']';
+  return v;
+}
+
+}  // namespace
+
+bool UpdateOp(const std::string& n, const std::vector<NDArray>& in, std::vector<NDArray>* outputs,
+              const Params& p) {
+  const Spec* spec = nullptr;
+  for (const Spec& s : kSpecs) {
+    if (n == s.name) spec = &s;
+  }
+  if (spec == nullptr) return false;
+  const int op = spec->op;
+  KV_CHECK_EQ(static_cast<int>(in.size()), spec->nin) << n << " expects " << spec->nin << " inputs";
+  const NDArray& w = in[0];
+  const NDArray& g = in[1];
+  for (const NDArray& a : in) {
+    KV_CHECK(a.stype() == kDefaultStorage)
+        << n << ": row_sparse weights, gradients or states are not supported (dense arrays only)";
+  }
+  KV_CHECK(w.on_gpu()) << n << " runs on GPU arrays only (no CPU fallback)";
+  const int dev = w.dev();
+  const int dtype = w.dtype();
+  if (op == kUpdMPNAG) {
+    KV_CHECK(dtype == kFloat16 || dtype == kBfloat16)
+        << n << ": the multi-precision form expects float16 / bfloat16 weights, got " << DTypeName(dtype);
+  } else {
+    KV_CHECK_EQ(dtype, kFloat32)
+        << n << ": " << DTypeName(dtype) << " weights without an fp32 master copy are not supported "
+        << "(float32 only; use multi_precision=True for 16-bit weights)";
+  }
+  for (const NDArray& a : in) {
+    KV_CHECK(a.on_gpu() && a.dev() == dev) << n << ": all operands must be on the same GPU";
+  }
+  KV_CHECK_EQ(g.dtype(), dtype) << n << ": weight / grad dtype mismatch";
+  KV_CHECK_EQ(g.Size(), w.Size()) << n << ": weight / grad shape mismatch";
+  for (int i = 2; i < spec->nin; ++i) {
+    KV_CHECK_EQ(in[i].dtype(), kFloat32) << n << ": optimizer states must be float32";
+    KV_CHECK_EQ(in[i].Size(), w.Size()) << n << ": state shape mismatch";
+  }
+  NDArray out;
+  if (outputs->empty()) {
+    out = NDArray(w.shape(), w.ctx(), dtype);
+    outputs->push_back(out);
+  } else {
+    out = (*outputs)[0];
+  }
+  KV_CHECK(out.on_gpu() && out.dev() == dev) << n << ": out must be on the weight's GPU";
+  KV_CHECK(out.stype() == kDefaultStorage) << n << ": out must be a dense array";
+  KV_CHECK_EQ(out.dtype(), dtype) << n << ": out dtype mismatch";
+  KV_CHECK_EQ(out.Size(), w.Size()) << n << ": out shape mismatch";
+  const bool out_is_w = out.SameStorage(w);
+  KV_CHECK(!out_is_w || out.data() == w.data()) << n << ": out overlaps the weight without being it";
+
+  UpdateLaunch L;
+  L.op = op;
+  L.dtype = dtype;
+  L.lr = Required(p, "lr", n);
+  L.wd = GetF(p, "wd", 0.f);
+  L.rescale = GetF(p, "rescale_grad", 1.0f);
+  L.clip = GetF(p, "clip_gradient", -1.0f);
+  switch (op) {
+    case kUpdNAG: case kUpdMPNAG:  // NAGMomParam
+      L.momentum = GetF(p, "momentum", 0.f);
+      break;
+    case kUpdSignSGD:  // SignSGDParam
+      break;
+    case kUpdSignum:  // SignumParam
+      L.momentum = GetF(p, "momentum", 0.f);
+      L.wd_lh = GetF(p, "wd_lh", 0.f);
+      break;
+    case kUpdRMSProp: case kUpdRMSPropAlex:  // RMSPropParam, RMSPropAlexParam
+      L.gamma1 = GetF(p, "gamma1", 0.95f);
+      L.gamma2 = GetF(p, "gamma2", 0.9f);
+      L.eps = GetF(p, "epsilon", 1e-8f);
+      L.clip_weights = GetF(p, "clip_weights", -1.0f);
+      break;
+    case kUpdFTML: {  // FTMLParam: epsilon is a double field, the clip field is clip_grad
+      L.beta1 = InRange(GetF(p, "beta1", 0.6f), "beta1", 0.f, 1.f);
+      L.beta2 = InRange(GetF(p, "beta2", 0.999f), "beta2", 0.f, 1.f);
+      const std::string* e = Find(p, "epsilon");
+      L.eps = static_cast<float>(e ? DmlcStod(*e) : static_cast<double>(1e-8f));
+      KV_CHECK(Find(p, "t") != nullptr) << "Required parameter t of " << n << " is missing";
+      const int t = GetI(p, "t", 0);
+      L.clip = GetF(p, "clip_grad", -1.0f);
+      // power::Map(beta, DType(t)) is ::powf of the host C library (math_functions-inl.h:58-61,126):
+      // evaluated here once per call rather than with the device's powf
+      L.p1 = ::powf(L.beta1, static_cast<float>(t));
+      L.p2 = ::powf(L.beta2, static_cast<float>(t));
+      break;
+    }
+    case kUpdFtrl:  // FtrlParam
+      L.lamda1 = GetF(p, "lamda1", 0.01f);
+      L.beta = GetF(p, "beta", 1.0f);
+      break;
+  }
+  L.w = w.data();
+  L.g = g.data();
+  L.out = out.data();
+  for (int i = 2; i < spec->nin; ++i) L.s[i - 2] = static_cast<float*>(in[i].data());
+  L.n = w.Size();
+  L.out_is_w = out_is_w;
+
+  Engine* eng = Engine::Get();
+  DeviceGuard guard(dev);
+  eng->BeginRead(dev, *g.var());
+  if (!out_is_w) eng->BeginRead(dev, *w.var());
+  eng->BeginWrite(dev, *out.var());
+  for (int i = 2; i < spec->nin; ++i) eng->BeginWrite(dev, *in[i].var());
+  LaunchUpdateOp(L, eng->Stream(dev));
+  eng->CountLaunch(spec->launch_name, static_cast<uint64_t>(spec->bytes_per_elem) * L.n);
+  const uint64_t seq = eng->Issue(dev);
+  eng->MarkRead(dev, seq, g.var());
+  if (!out_is_w) eng->MarkRead(dev, seq, w.var());
+  eng->MarkWrite(dev, seq, out.var());
+  for (int i = 2; i < spec->nin; ++i) eng->MarkWrite(dev, seq, in[i].var());
+  return true;
+}
+
+}  // namespace b200kv

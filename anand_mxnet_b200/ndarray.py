@@ -534,6 +534,16 @@ multi_sgd_mom_update = _op('multi_sgd_mom_update')
 multi_mp_sgd_update = _op('multi_mp_sgd_update')
 multi_mp_sgd_mom_update = _op('multi_mp_sgd_mom_update')
 adam_update = _op('adam_update')
+# the operators of the reference's NAG / Signum / RMSProp / FTML / Ftrl optimizers (dense float32;
+# mp_nag_mom_update: float16 / bfloat16 weights with float32 mom and weight32)
+nag_mom_update = _op('nag_mom_update')
+mp_nag_mom_update = _op('mp_nag_mom_update')
+signsgd_update = _op('signsgd_update')
+signum_update = _op('signum_update')
+rmsprop_update = _op('rmsprop_update')
+rmspropalex_update = _op('rmspropalex_update')
+ftml_update = _op('ftml_update')
+ftrl_update = _op('ftrl_update')
 cast = _op('cast')
 multi_sum_sq = _op('multi_sum_sq')
 multi_lars = _op('multi_lars')
