@@ -206,7 +206,7 @@ void LaunchMultiLars(int n, float* out, const float* lrs, const float* wsq, cons
 // nag_mom_update, mp_nag_mom_update, signsgd_update, signum_update, rmsprop_update,
 // rmspropalex_update, ftml_update, ftrl_update (optimizer_op-inl.h:1061-1222, 1953-2158, 2344-2431)
 enum UpdOp : int { kUpdNAG = 0, kUpdMPNAG, kUpdSignSGD, kUpdSignum, kUpdRMSProp, kUpdRMSPropAlex,
-                   kUpdFTML, kUpdFtrl };
+                   kUpdFTML, kUpdFtrl, kUpdAdaGrad };
 struct UpdateLaunch {
   int op = kUpdNAG;
   int dtype = 0;                 // of w / g / out: kFloat32, or kFloat16 / kBfloat16 for kUpdMPNAG
@@ -221,8 +221,18 @@ struct UpdateLaunch {
   float lr = 0.f, wd = 0.f, rescale = 1.f, clip = -1.f, momentum = 0.f, wd_lh = 0.f, gamma1 = 0.f,
         gamma2 = 0.f, eps = 0.f, clip_weights = -1.f, beta1 = 0.f, beta2 = 0.f, p1 = 0.f, p2 = 0.f,
         lamda1 = 0.f, beta = 0.f;
+  // row_sparse forms (LaunchRspRowUpdateOp): w / out / s hold every row of the table, g holds
+  // `nnr` rows of `row_len` elements, and gradient row r updates table row gidx[r]
+  const int64_t* gidx = nullptr;
+  int64_t nnr = 0, row_len = 0;
 };
 void LaunchUpdateOp(const UpdateLaunch& L, cudaStream_t stream);
+// row_sparse forms of ftrl_update and _sparse_adagrad_update (rowsparse_kernels.cu;
+// FtrlDnsRspDnsKernel, AdagradDnsRspDnsKernel: optimizer_op-inl.h:2186-2219, 2507-2531): float32,
+// one warp per gradient row, the same Step<OP> as the dense kernel. Rows not in gidx stay untouched.
+void LaunchRspRowUpdateOp(const UpdateLaunch& L, cudaStream_t stream);
+// FillDnsZerosRspImpl's id half (init_op.h:474-487): ids[i] = i for i < rows
+void LaunchFillRowIds(int64_t* ids, int64_t rows, cudaStream_t stream);
 
 // ---- 2-bit gradient compression with residual (compress_kernels.cu;
 // src/kvstore/gradient_compression-inl.h:40-132, comm.h:552-596 ReduceCompressed) ----

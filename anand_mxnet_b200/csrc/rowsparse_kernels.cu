@@ -105,6 +105,72 @@ __global__ void __launch_bounds__(kWarpsPerBlock * 32) rsp_update_kernel(RspUpda
   }
 }
 
+// row_sparse forms of the callback route's operators (ftrl_update, _sparse_adagrad_update): one
+// warp per gradient row in a grid-stride loop, the row id read once per row, then the row's
+// elements through the same Step<OP> as the dense update_kernel; out is the weight itself
+template <int OP>
+__global__ void __launch_bounds__(kWarpsPerBlock * 32) rsp_row_update_kernel(const UpdateLaunch a,
+                                                                              const bool vec) {
+  constexpr int NS = NumStates(OP);
+  const int lane = threadIdx.x & 31;
+  const int64_t nwarps = static_cast<int64_t>(gridDim.x) * kWarpsPerBlock;
+  const int64_t len = a.row_len;
+  for (int64_t r = static_cast<int64_t>(blockIdx.x) * kWarpsPerBlock + (threadIdx.x >> 5); r < a.nnr;
+       r += nwarps) {
+    const int64_t off = a.gidx[r] * len;
+    const float* g = static_cast<const float*>(a.g) + r * len;
+    float* w = static_cast<float*>(a.out) + off;
+    float* s[NS];
+#pragma unroll
+    for (int k = 0; k < NS; ++k) s[k] = a.s[k] + off;
+    if (vec) {
+      for (int64_t v = lane; v < len / 4; v += 32) {
+        const float4 g4 = __ldcs(reinterpret_cast<const float4*>(g) + v);
+        const float4 w4 = reinterpret_cast<const float4*>(w)[v];
+        float4 s4[NS];
+#pragma unroll
+        for (int k = 0; k < NS; ++k) s4[k] = reinterpret_cast<const float4*>(s[k])[v];
+        const float gx[4] = {g4.x, g4.y, g4.z, g4.w}, wx[4] = {w4.x, w4.y, w4.z, w4.w};
+        float o[4], sx[NS][4];
+#pragma unroll
+        for (int k = 0; k < NS; ++k) {
+          sx[k][0] = s4[k].x; sx[k][1] = s4[k].y; sx[k][2] = s4[k].z; sx[k][3] = s4[k].w;
+        }
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+          float st[3] = {0.f, 0.f, 0.f};
+#pragma unroll
+          for (int k = 0; k < NS; ++k) st[k] = sx[k][j];
+          o[j] = Step<OP>(a, wx[j], gx[j], st);
+#pragma unroll
+          for (int k = 0; k < NS; ++k) sx[k][j] = st[k];
+        }
+        reinterpret_cast<float4*>(w)[v] = make_float4(o[0], o[1], o[2], o[3]);
+#pragma unroll
+        for (int k = 0; k < NS; ++k) {
+          reinterpret_cast<float4*>(s[k])[v] = make_float4(sx[k][0], sx[k][1], sx[k][2], sx[k][3]);
+        }
+      }
+    } else {
+      for (int64_t j = lane; j < len; j += 32) {
+        float st[3] = {0.f, 0.f, 0.f};
+#pragma unroll
+        for (int k = 0; k < NS; ++k) st[k] = s[k][j];
+        w[j] = Step<OP>(a, w[j], __ldcs(g + j), st);
+#pragma unroll
+        for (int k = 0; k < NS; ++k) s[k][j] = st[k];
+      }
+    }
+  }
+}
+
+__global__ void fill_row_ids_kernel(int64_t* ids, int64_t rows) {
+  const int64_t stride = static_cast<int64_t>(gridDim.x) * blockDim.x;
+  for (int64_t i = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x; i < rows; i += stride) {
+    ids[i] = i;
+  }
+}
+
 // ---------------------------------------------------------------------------------------------
 // push: union + ordered sum
 
@@ -828,6 +894,29 @@ void LaunchRspUpdate(const RspUpdateLaunch& p, cudaStream_t stream) {
     case kOptAdam: rsp_update_kernel<kOptAdam><<<blocks, kWarpsPerBlock * 32, 0, stream>>>(p); break;
     default: KV_FATAL << "row_sparse update: unsupported optimizer kind " << p.opt;
   }
+  KV_CUDA(cudaGetLastError());
+}
+
+void LaunchRspRowUpdateOp(const UpdateLaunch& L, cudaStream_t stream) {
+  if (L.nnr <= 0 || L.row_len <= 0) return;
+  KV_CHECK_EQ(L.dtype, kFloat32) << "row_sparse optimizer operators run on float32 arrays";
+  KV_CHECK(L.out == L.w) << "row_sparse optimizer operators update the weight in place";
+  auto aligned = [](const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; };
+  bool vec = L.row_len % 4 == 0 && aligned(L.g) && aligned(L.out);
+  for (int k = 0; k < NumStates(L.op); ++k) vec = vec && aligned(L.s[k]);
+  const int blocks = static_cast<int>(std::min<int64_t>((L.nnr + kWarpsPerBlock - 1) / kWarpsPerBlock,
+                                                        kNumSMs * 16));
+  switch (L.op) {
+    case kUpdFtrl: rsp_row_update_kernel<kUpdFtrl><<<blocks, kWarpsPerBlock * 32, 0, stream>>>(L, vec); break;
+    case kUpdAdaGrad: rsp_row_update_kernel<kUpdAdaGrad><<<blocks, kWarpsPerBlock * 32, 0, stream>>>(L, vec); break;
+    default: KV_FATAL << "row_sparse optimizer operator: unsupported operator " << L.op;
+  }
+  KV_CUDA(cudaGetLastError());
+}
+
+void LaunchFillRowIds(int64_t* ids, int64_t rows, cudaStream_t stream) {
+  if (rows <= 0) return;
+  fill_row_ids_kernel<<<GridFor(rows, 256), 256, 0, stream>>>(ids, rows);
   KV_CUDA(cudaGetLastError());
 }
 

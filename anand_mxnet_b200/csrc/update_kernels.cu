@@ -4,14 +4,16 @@
 //
 // One elementwise kernel update_kernel<OP, T> over one flat tensor: a grid-stride loop whose body
 // moves 16 bytes per operand (float4, or 8 x 16 bit) when every operand is 16-byte aligned, and a
-// scalar loop for the rest (unaligned slices, the tail). Each Step<OP> follows the expression tree
-// of the reference's CPU kernel as written (src/operator/optimizer_op-inl.h), one explicitly
-// rounded IEEE operation per node, so the results equal the reference's bit for bit.
+// scalar loop for the rest (unaligned slices, the tail). Each Step<OP> (opt_math.cuh, shared with
+// the row_sparse forms in rowsparse_kernels.cu) follows the expression tree of the reference's CPU
+// kernel as written (src/operator/optimizer_op-inl.h), one explicitly rounded IEEE operation per
+// node, so the results equal the reference's bit for bit.
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
 
 #include "common.h"
 #include "kernels.h"
+#include "opt_math.cuh"
 
 namespace b200kv {
 namespace {
@@ -27,100 +29,6 @@ template <typename T> __device__ __forceinline__ T FromF(float x);
 template <> __device__ __forceinline__ float FromF<float>(float x) { return x; }
 template <> __device__ __forceinline__ __half FromF<__half>(float x) { return __float2half_rn(x); }
 template <> __device__ __forceinline__ __nv_bfloat16 FromF<__nv_bfloat16>(float x) { return __float2bfloat16_rn(x); }
-
-// fp32 state arrays of each operator (input order after weight, grad) and whether it reads weight
-__host__ __device__ constexpr int NumStates(int op) {
-  return op == kUpdSignSGD ? 0
-         : (op == kUpdNAG || op == kUpdSignum || op == kUpdRMSProp) ? 1
-         : (op == kUpdMPNAG || op == kUpdFtrl) ? 2 : 3;
-}
-__host__ __device__ constexpr bool ReadsWeight(int op) { return op != kUpdMPNAG; }
-
-// mshadow_op::clip::Map (mshadow_op.h:912-922)
-__device__ __forceinline__ float Clip(float x, float b) { return x > b ? b : (x < -b ? -b : x); }
-// (x > 0) - (x < 0): an int, 0 for NaN
-__device__ __forceinline__ float SignInt(float x) { return static_cast<float>((x > 0.f) - (x < 0.f)); }
-
-// One element. w: weight (unused by mp_nag), g: gradient, s: the states, updated in place.
-// Returns the value stored to out.
-template <int OP>
-__device__ __forceinline__ float Step(const UpdateLaunch& a, float w, float g, float (&s)[3]) {
-  if (OP == kUpdNAG || OP == kUpdMPNAG) {
-    // NAGMomKernel / MP_NAGMomKernel (optimizer_op-inl.h:1061-1138): mom = momentum*mom first;
-    // out = (w - mom) + (momentum+1)*(mom - lr*(clip(rescale*g) + wd*w)); then
-    // mom = mom - lr*(clip(rescale*g) + wd*w') where w' is the weight as it reads after out was
-    // stored: the new value for mp_nag (a local) and for nag when out is the weight itself
-    const float w0 = OP == kUpdMPNAG ? s[1] : w;
-    float cg = __fmul_rn(a.rescale, g);
-    if (a.clip >= 0.f) cg = Clip(cg, a.clip);
-    const float mom = __fmul_rn(a.momentum, s[0]);
-    const float out = __fadd_rn(__fsub_rn(w0, mom),
-                                __fmul_rn(__fadd_rn(a.momentum, 1.f),
-                                          __fsub_rn(mom, __fmul_rn(a.lr, __fadd_rn(cg, __fmul_rn(a.wd, w0))))));
-    const float w1 = (OP == kUpdMPNAG || a.out_is_w) ? out : w0;
-    s[0] = __fsub_rn(mom, __fmul_rn(a.lr, __fadd_rn(cg, __fmul_rn(a.wd, w1))));
-    if (OP == kUpdMPNAG) s[1] = out;
-    return out;
-  }
-  if (OP == kUpdSignSGD) {
-    // SignSGDKernel (2344-2356): clip_gradient and rescale_grad have no effect
-    return __fsub_rn(__fmul_rn(__fsub_rn(1.f, __fmul_rn(a.lr, a.wd)), w), __fmul_rn(a.lr, SignInt(g)));
-  }
-  if (OP == kUpdSignum) {
-    // SignumKernel (2412-2431): the clipped branch multiplies (1-momentum) by clip(rescale*g), the
-    // other one ((1-momentum)*rescale)*g
-    const float om = __fsub_rn(1.f, a.momentum);
-    const float t = a.clip >= 0.f ? __fmul_rn(om, Clip(__fmul_rn(a.rescale, g), a.clip))
-                                  : __fmul_rn(__fmul_rn(om, a.rescale), g);
-    s[0] = __fsub_rn(__fsub_rn(__fmul_rn(a.momentum, s[0]), __fmul_rn(__fmul_rn(om, a.wd), w)), t);
-    return __fadd_rn(__fmul_rn(__fsub_rn(1.f, __fmul_rn(a.lr, a.wd_lh)), w), __fmul_rn(a.lr, SignInt(s[0])));
-  }
-  if (OP == kUpdRMSProp || OP == kUpdRMSPropAlex) {
-    // RMSPropUpdateKernel (2052-2077), RMSPropAlexUpdateKernel (1953-1986): wd*w joins the
-    // gradient before the clip
-    float gr = __fadd_rn(__fmul_rn(a.rescale, g), __fmul_rn(a.wd, w));
-    if (a.clip >= 0.f) gr = Clip(gr, a.clip);
-    const float om = __fsub_rn(1.f, a.gamma1);
-    float r;
-    if (OP == kUpdRMSProp) {
-      s[0] = __fadd_rn(__fmul_rn(om, __fmul_rn(gr, gr)), __fmul_rn(a.gamma1, s[0]));
-      r = __fsub_rn(w, __fmul_rn(a.lr, __fdiv_rn(gr, __fsqrt_rn(__fadd_rn(s[0], a.eps)))));
-    } else {
-      s[0] = __fadd_rn(__fmul_rn(__fmul_rn(om, gr), gr), __fmul_rn(a.gamma1, s[0]));
-      s[1] = __fadd_rn(__fmul_rn(om, gr), __fmul_rn(a.gamma1, s[1]));
-      s[2] = __fsub_rn(__fmul_rn(a.gamma2, s[2]),
-                       __fdiv_rn(__fmul_rn(a.lr, gr),
-                                 __fsqrt_rn(__fadd_rn(__fsub_rn(s[0], __fmul_rn(s[1], s[1])), a.eps))));
-      r = __fadd_rn(w, s[2]);
-    }
-    return a.clip_weights >= 0.f ? Clip(r, a.clip_weights) : r;
-  }
-  if (OP == kUpdFTML) {
-    // FTMLKernel (1205-1222), states d, v, z; p1 = powf(beta1, t), p2 = powf(beta2, t)
-    float gi = __fadd_rn(__fmul_rn(a.rescale, g), __fmul_rn(a.wd, w));
-    if (a.clip >= 0.f) gi = Clip(gi, a.clip);
-    s[1] = __fadd_rn(__fmul_rn(a.beta2, s[1]), __fmul_rn(__fsub_rn(1.f, a.beta2), __fmul_rn(gi, gi)));
-    const float dt = __fmul_rn(__fdiv_rn(__fsub_rn(1.f, a.p1), a.lr),
-                               __fadd_rn(__fsqrt_rn(__fdiv_rn(s[1], __fsub_rn(1.f, a.p2))), a.eps));
-    s[2] = __fsub_rn(__fadd_rn(__fmul_rn(a.beta1, s[2]), __fmul_rn(__fsub_rn(1.f, a.beta1), gi)),
-                     __fmul_rn(__fsub_rn(dt, __fmul_rn(a.beta1, s[0])), w));
-    s[0] = dt;
-    return __fdiv_rn(-s[2], dt);
-  }
-  // FtrlUpdateKernel (2133-2158), states z, n: z is updated before n; the result is MULTIPLIED by
-  // gt(|z|, lamda1), so it is -0.0 for -lamda1 < z < 0 and NaN when the quotient is infinite
-  float gr = __fmul_rn(g, a.rescale);
-  if (a.clip >= 0.f) gr = Clip(gr, a.clip);
-  const float g2 = __fmul_rn(gr, gr);
-  s[0] = __fadd_rn(s[0], __fsub_rn(gr, __fdiv_rn(__fmul_rn(__fsub_rn(__fsqrt_rn(__fadd_rn(s[1], g2)),
-                                                                    __fsqrt_rn(s[1])), w), a.lr)));
-  s[1] = __fadd_rn(s[1], g2);
-  const float z = s[0];
-  const float sgn = z < 0.f ? -1.f : (z > 0.f ? 1.f : 0.f);  // mshadow_op::sign
-  return __fmul_rn(__fdiv_rn(__fsub_rn(__fmul_rn(sgn, a.lamda1), z),
-                             __fadd_rn(__fdiv_rn(__fadd_rn(a.beta, __fsqrt_rn(s[1])), a.lr), a.wd)),
-                   fabsf(z) > a.lamda1 ? 1.f : 0.f);
-}
 
 // V consecutive elements of a 16-byte group, as floats
 template <typename T, int V>

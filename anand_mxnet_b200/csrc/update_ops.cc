@@ -1,17 +1,21 @@
 // update_ops.cc -- host side of the single-tensor optimizer operators that the reference's NAG,
 // Signum, RMSProp, FTML and Ftrl optimizers call from their `update` (the per-key updater callback
-// of the store, and the local updaters of update_on_kvstore=False). Kernels: update_kernels.cu.
+// of the store, and the local updaters of update_on_kvstore=False), plus the row_sparse forms of
+// ftrl_update and AdaGrad's _sparse_adagrad_update. Kernels: update_kernels.cu (dense),
+// rowsparse_kernels.cu (row_sparse).
 //
 // Reference operator definitions (inputs, parameter structs, kernels):
 //   nag_mom_update, mp_nag_mom_update    src/operator/optimizer_op.cc:712-762, optimizer_op-inl.h:1032-1160
 //   ftml_update                          optimizer_op.cc:626-660, optimizer_op-inl.h:1163-1249
 //   rmsprop_update, rmspropalex_update   optimizer_op.cc:763-853, optimizer_op-inl.h:1915-2099
-//   ftrl_update                          optimizer_op.cc:854-890, optimizer_op-inl.h:2101-2183
+//   ftrl_update, _sparse_ftrl_update     optimizer_op.cc:854-893, optimizer_op-inl.h:2101-2314
 //   signsgd_update, signum_update        optimizer_op.cc:49-104, optimizer_op-inl.h:2319-2452
+//   _sparse_adagrad_update               optimizer_op.cc:895-924, optimizer_op-inl.h:2454-2649
 //
-// Dense float32 arrays only (mp_nag_mom_update: float16 / bfloat16 weights with float32 mom and
-// weight32). The reference would densify a row_sparse gradient and run 16-bit weights of the other
-// operators in half precision; both are refused here before anything is launched.
+// Dense float32 arrays (mp_nag_mom_update: float16 / bfloat16 weights with float32 mom and
+// weight32), or the row_sparse forms in float32 (RspUpdateOp). The reference would densify a
+// row_sparse gradient of a dense-weight ftrl_update and run 16-bit weights of the other operators
+// in half precision; both are refused here before anything is launched.
 #include <cctype>
 #include <cerrno>
 #include <cmath>
@@ -41,6 +45,10 @@ const Spec kSpecs[] = {
     {"rmspropalex_update", kUpdRMSPropAlex, 5, "update_op(rmspropalex_update)", 36},
     {"ftml_update", kUpdFTML, 5, "update_op(ftml_update)", 36},
     {"ftrl_update", kUpdFtrl, 4, "update_op(ftrl_update)", 28},
+    // row_sparse only: the alias of ftrl_update (MXNET_ADD_SPARSE_OP_ALIAS, optimizer_op.cc:855)
+    // and AdaGrad's operator (optimizer_op.cc:895-924, optimizer_op-inl.h:2454-2649)
+    {"_sparse_ftrl_update", kUpdFtrl, 4, "update_op(ftrl_update)", 28},
+    {"_sparse_adagrad_update", kUpdAdaGrad, 3, "update_op(_sparse_adagrad_update)", 20},
 };
 
 // Restatement of dmlc::stod == ParseFloat<double, true> (3rdparty/dmlc-core/include/dmlc/
@@ -138,6 +146,109 @@ float InRange(float v, const char* key, float lo, float hi) {
   return v;
 }
 
+const char* StypeName(int stype) { return stype == kRowSparseStorage ? "row_sparse" : "default"; }
+
+// ftrl_update (FtrlUpdateEx, optimizer_op-inl.h:2291-2314) and _sparse_adagrad_update
+// (AdagradStorageType / AdagradUpdateEx, 2480-2501, 2620-2649) with row_sparse operands: only the
+// rows listed in the gradient move. Every check runs before anything is enqueued, so a refused
+// call leaves all operands as they were. Accepted forms:
+//   ftrl_update / _sparse_ftrl_update   (row_sparse weight, grad, z, n)
+//   _sparse_adagrad_update              (row_sparse weight, grad, history), wd == 0
+//                                       (dense weight, row_sparse grad, dense history), wd == 0
+void RspUpdateOp(const Spec& spec, const std::vector<NDArray>& in, std::vector<NDArray>* outputs,
+                 const Params& p) {
+  const std::string n = spec.name;
+  const int op = spec.op;
+  const NDArray& w = in[0];
+  const NDArray& g = in[1];
+  const int wst = w.stype();
+  UpdateLaunch L;
+  L.op = op;
+  L.dtype = kFloat32;
+  L.lr = Required(p, "lr", n);
+  L.wd = GetF(p, "wd", 0.f);
+  L.rescale = GetF(p, "rescale_grad", 1.0f);
+  L.clip = GetF(p, "clip_gradient", -1.0f);
+  if (op == kUpdFtrl) {  // FtrlParam
+    L.lamda1 = GetF(p, "lamda1", 0.01f);
+    L.beta = GetF(p, "beta", 1.0f);
+    KV_CHECK(wst == kRowSparseStorage && g.stype() == kRowSparseStorage)
+        << n << ": the row_sparse form needs row_sparse weight, grad, z and n (a dense weight with a "
+        << "row_sparse gradient is not supported)";
+  } else {  // AdagradParam; AdagradUpdateDnsRspDnsImpl (2569-2570) checks wd first
+    L.eps = GetF(p, "epsilon", 1.0e-7f);
+    KV_CHECK(L.wd == 0.f) << "sparse adagrad_update does not support wd.";
+    KV_CHECK(g.stype() == kRowSparseStorage && in[2].stype() == wst)
+        << n << ": supported storage types are (row_sparse, row_sparse, row_sparse) and (default, "
+        << "row_sparse, default), got (" << StypeName(wst) << ", " << StypeName(g.stype()) << ", "
+        << StypeName(in[2].stype()) << ")";
+  }
+  for (const NDArray& a : in) {
+    KV_CHECK(a.on_gpu() && a.dev() == w.dev()) << n << ": all operands must be on the same GPU";
+    KV_CHECK_EQ(a.dtype(), kFloat32) << n << ": row_sparse updates run on float32 arrays only, got "
+                                     << DTypeName(a.dtype());
+    KV_CHECK(a.shape() == w.shape()) << n << ": weight / grad / state shape mismatch";
+  }
+  KV_CHECK(!w.shape().empty()) << n << ": the weight needs at least one dimension";
+  const int64_t rows = w.shape()[0];
+  // CheckAllRowsPresent (operator_common.h:500-511)
+  const char* func = op == kUpdFtrl ? "FtrlUpdate" : "AdagradUpdate";
+  KV_CHECK(wst != kRowSparseStorage || w.nnr() == rows)
+      << func << " for RowSparse weights is only implemented for RowSparse weights with all rows "
+      << "containing non-zeros. Expects weights.data.shape[0] (" << w.nnr() << ") == weights.shape[0] ("
+      << rows << ").";
+  // the states' rows are addressed by the table row id, like the weight's: a row_sparse state holds
+  // every row, or none yet (then it is zero-filled first, FillDnsZerosRspImpl)
+  for (size_t i = 2; i < in.size(); ++i) {
+    KV_CHECK(in[i].stype() != kRowSparseStorage || in[i].nnr() == 0 || in[i].nnr() == rows)
+        << n << ": a row_sparse optimizer state must hold every row or none (it holds "
+        << in[i].nnr() << " of " << rows << ")";
+  }
+  // kWriteInplace is expected (optimizer_op-inl.h:2235, 2572)
+  KV_CHECK(outputs->size() == 1 && (*outputs)[0].SameStorage(w) && (*outputs)[0].stype() == wst &&
+           (*outputs)[0].data() == w.data())
+      << n << ": out must be the weight itself (kWriteInplace is expected for sparse " << spec.name
+      << ")";
+
+  const int dev = w.dev();
+  Engine* eng = Engine::Get();
+  DeviceGuard guard(dev);
+  std::vector<const NDArray*> fill;
+  for (size_t i = 2; i < in.size(); ++i) {
+    if (in[i].stype() == kRowSparseStorage && in[i].nnr() == 0) {
+      in[i].CheckAndAllocRows(rows);
+      fill.push_back(&in[i]);
+    }
+  }
+  const bool update = g.storage_initialized();
+  if (!update && fill.empty()) return;  // an all-zero gradient changes nothing
+  if (update) eng->BeginRead(dev, *g.var());
+  eng->BeginWrite(dev, *w.var());
+  for (size_t i = 2; i < in.size(); ++i) eng->BeginWrite(dev, *in[i].var());
+  cudaStream_t st = eng->Stream(dev);
+  for (const NDArray* a : fill) {
+    KV_CUDA(cudaMemsetAsync(a->data(), 0, static_cast<size_t>(rows) * a->RowLength() * sizeof(float), st));
+    LaunchFillRowIds(a->row_ids(), rows, st);
+    eng->CountLaunch(spec.launch_name, static_cast<uint64_t>(rows) * (a->RowLength() * 4 + 8));
+  }
+  if (update) {
+    L.w = w.data();
+    L.out = w.data();
+    L.g = g.data();
+    L.gidx = g.row_ids();
+    L.nnr = g.nnr();
+    L.row_len = static_cast<int64_t>(w.RowLength());
+    for (size_t i = 2; i < in.size(); ++i) L.s[i - 2] = static_cast<float*>(in[i].data());
+    LaunchRspRowUpdateOp(L, st);
+    eng->CountLaunch(spec.launch_name,
+                     static_cast<uint64_t>(L.nnr) * (spec.bytes_per_elem * L.row_len + 8));
+  }
+  const uint64_t seq = eng->Issue(dev);
+  if (update) eng->MarkRead(dev, seq, g.var());
+  eng->MarkWrite(dev, seq, w.var());
+  for (size_t i = 2; i < in.size(); ++i) eng->MarkWrite(dev, seq, in[i].var());
+}
+
 }  // namespace
 
 bool UpdateOp(const std::string& n, const std::vector<NDArray>& in, std::vector<NDArray>* outputs,
@@ -151,6 +262,17 @@ bool UpdateOp(const std::string& n, const std::vector<NDArray>& in, std::vector<
   KV_CHECK_EQ(static_cast<int>(in.size()), spec->nin) << n << " expects " << spec->nin << " inputs";
   const NDArray& w = in[0];
   const NDArray& g = in[1];
+  if (op == kUpdFtrl) {  // FtrlUpdateEx (optimizer_op-inl.h:2303-2306)
+    for (int i : {2, 3}) {
+      KV_CHECK(in[i].stype() == w.stype())
+          << "Inconsistent storage type detected between  " << (i == 2 ? "z" : "n") << ".stype = "
+          << in[i].stype() << " and weight.stype = " << w.stype();
+    }
+  }
+  if (op == kUpdAdaGrad || w.stype() == kRowSparseStorage) {
+    RspUpdateOp(*spec, in, outputs, p);
+    return true;
+  }
   for (const NDArray& a : in) {
     KV_CHECK(a.stype() == kDefaultStorage)
         << n << ": row_sparse weights, gradients or states are not supported (dense arrays only)";

@@ -544,6 +544,12 @@ rmsprop_update = _op('rmsprop_update')
 rmspropalex_update = _op('rmspropalex_update')
 ftml_update = _op('ftml_update')
 ftrl_update = _op('ftrl_update')
+# mx.nd.sparse.*: lazy row updates over the rows of a row_sparse gradient (float32, out must be the
+# weight): ftrl_update on row_sparse weight / grad / z / n (mx.nd.ftrl_update takes the same form
+# from its operands' storage types), adagrad_update on (row_sparse, row_sparse, row_sparse) or
+# (dense, row_sparse, dense) with wd = 0
+_Sparse.ftrl_update = staticmethod(_op('_sparse_ftrl_update'))
+_Sparse.adagrad_update = staticmethod(_op('_sparse_adagrad_update'))
 cast = _op('cast')
 multi_sum_sq = _op('multi_sum_sq')
 multi_lars = _op('multi_lars')
