@@ -561,12 +561,13 @@ int PushExternal(void (*async_fn)(void*, void*, void*), void (*sync_fn)(void*, v
     }
   }
   const bool gpu = ctx.dev_type == kGPU;
-  const int lane = gpu ? ctx.dev_id : -1;
   RunCtxABI rctx{ctx.dev_type, ctx.dev_id, nullptr, nullptr, false};
+  std::unique_ptr<LaneOp> op;
   if (gpu) {
-    for (Var* v : rd) eng->BeginRead(lane, *v);
-    for (Var* v : wr) eng->BeginWrite(lane, *v);
-    rctx.stream = eng->Stream(lane);
+    op.reset(new LaneOp(ctx.dev_id));
+    for (Var* v : rd) op->Read(v);
+    for (Var* v : wr) op->Write(v);
+    rctx.stream = op->stream();
   } else {
     for (Var* v : rd) eng->WaitToRead(*v);
     for (Var* v : wr) eng->WaitToWrite(*v);
@@ -585,11 +586,7 @@ int PushExternal(void (*async_fn)(void*, void*, void*), void (*sync_fn)(void*, v
     pend.failed = true;
     pend.msg = e.what();
   }
-  if (gpu) {
-    const uint64_t seq = eng->Issue(lane);
-    for (Var* v : rd) eng->MarkRead(lane, seq, v);
-    for (Var* v : wr) eng->MarkWrite(lane, seq, v);
-  }
+  if (op) op->Issue();
   if (pend.failed) {
     const std::string msg = std::string("operator ") + (opr_name ? opr_name : "<external>") + ": " + pend.msg;
     for (Var* w : wr) eng->SetError(w, msg);

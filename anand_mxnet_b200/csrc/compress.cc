@@ -20,7 +20,6 @@ void KVStore::CompressedReduceGroup(const std::vector<KeyEntry*>& es, std::vecto
   Engine* eng = Engine::Get();
   const int dev = g->dev(), W = g->world();
   DeviceGuard guard(dev);
-  cudaStream_t st = eng->Stream(dev);
   std::vector<int64_t> mine;
   for (size_t k = 0; k < es.size(); ++k) {
     KeyEntry& e = *es[k];
@@ -41,24 +40,17 @@ void KVStore::CompressedReduceGroup(const std::vector<KeyEntry*>& es, std::vecto
     }
     NDArray& res = e.gc_residual[0];
     if (res.is_none()) {
-      res = NDArray(e.shape, Context::GPU(dev), kFloat32);
-      eng->BeginWrite(dev, *res.var());
-      KV_CUDA(cudaMemsetAsync(res.data(), 0, res.ByteSize(), st));
-      eng->MarkWrite(dev, eng->Issue(dev), res.var());
+      res = ZerosOn(e.shape, dev, kFloat32);
       e.gc_compressed[0] = NDArray({words}, Context::GPU(dev), kInt32);
       KV_CHECK(g->InArena(e.gc_compressed[0].data())) << "IPC arena exhausted; raise B200KV_IPC_ARENA_MB";
     }
     NDArray& comp = e.gc_compressed[0];
-    eng->BeginRead(dev, *src.var());
-    eng->BeginWrite(dev, *res.var());
-    eng->BeginWrite(dev, *comp.var());
+    LaneOp op(dev);
+    op.Read(src).Write(res).Write(comp);
     LaunchQuantize2Bit(static_cast<const float*>(src.data()), static_cast<float*>(res.data()),
-                       static_cast<uint32_t*>(comp.data()), n, gc_threshold_, st);
+                       static_cast<uint32_t*>(comp.data()), n, gc_threshold_, op.stream());
     eng->CountLaunch("quantize_2bit", n * 12 + words * 4);
-    const uint64_t seq = eng->Issue(dev);
-    eng->MarkRead(dev, seq, src.var());
-    eng->MarkWrite(dev, seq, res.var());
-    eng->MarkWrite(dev, seq, comp.var());
+    op.Issue();
     mine.push_back(e.key);
     mine.push_back(static_cast<int64_t>(n));
     mine.push_back(g->OffsetOf(comp.data()));
@@ -75,10 +67,12 @@ void KVStore::CompressedReduceGroup(const std::vector<KeyEntry*>& es, std::vecto
       ptrs[r] = static_cast<const uint32_t*>(g->PeerPtr(r, f[2]));
     }
     if (e.gc_merged.is_none()) e.gc_merged = NDArray(e.shape, Context::GPU(dev), kFloat32);
-    eng->BeginWrite(dev, *e.gc_merged.var());
-    LaunchDequantizeSum2Bit(ptrs.data(), W, static_cast<float*>(e.gc_merged.data()), e.size, gc_threshold_, st);
+    LaneOp op(dev);
+    op.Write(e.gc_merged);
+    LaunchDequantizeSum2Bit(ptrs.data(), W, static_cast<float*>(e.gc_merged.data()), e.size, gc_threshold_,
+                            op.stream());
     eng->CountLaunch("dequantize_sum_2bit", e.size * 4 + static_cast<uint64_t>(W) * ((e.size + 15) / 16) * 4);
-    eng->MarkWrite(dev, eng->Issue(dev), e.gc_merged.var());
+    op.Issue();
     (*srcs)[k].assign(1, e.gc_merged);
   }
   GroupBarrier();   // the peers have read my words: the next quantise may overwrite them
@@ -113,52 +107,35 @@ NDArray KVStore::CompressedReduce(KeyEntry& e, const std::vector<NDArray>& srcs_
     if (std::find(parts.begin(), parts.end(), d) == parts.end()) parts.push_back(d);
     NDArray& res = e.gc_residual[i];
     if (res.is_none() || res.dev() != d) {
-      // buf.residual[i] = 0 on the source's device (comm.h:569-571)
-      res = NDArray(e.shape, Context::GPU(d), kFloat32);
-      DeviceGuard g(d);
-      eng->BeginWrite(d, *res.var());   // first writer of a possibly recycled block
-      KV_CUDA(cudaMemsetAsync(res.data(), 0, res.ByteSize(), eng->Stream(d)));
-      eng->MarkWrite(d, eng->Issue(d), res.var());
+      res = ZerosOn(e.shape, d, kFloat32);   // buf.residual[i] = 0 on the source's device (comm.h:569-571)
       e.gc_compressed[i] = NDArray({words}, Context::GPU(d), kInt32);
     }
     NDArray& comp = e.gc_compressed[i];
     // quantise where the gradient lives: what crosses NVLink afterwards is 1/16 of it
-    eng->BeginRead(d, *src.var());
-    eng->BeginWrite(d, *res.var());
-    eng->BeginWrite(d, *comp.var());
-    {
-      DeviceGuard g(d);
-      LaunchQuantize2Bit(static_cast<const float*>(src.data()), static_cast<float*>(res.data()),
-                         static_cast<uint32_t*>(comp.data()), n, gc_threshold_, eng->Stream(d));
-    }
+    LaneOp op(d);
+    op.Read(src).Write(res).Write(comp);
+    LaunchQuantize2Bit(static_cast<const float*>(src.data()), static_cast<float*>(res.data()),
+                       static_cast<uint32_t*>(comp.data()), n, gc_threshold_, op.stream());
     eng->CountLaunch("quantize_2bit", n * 12 + words * 4);
-    const uint64_t seq = eng->Issue(d);
-    eng->MarkRead(d, seq, src.var());
-    eng->MarkWrite(d, seq, res.var());
-    eng->MarkWrite(d, seq, comp.var());
+    op.Issue();
     comp_ptrs[i] = static_cast<const uint32_t*>(comp.data());
   }
   if (parts.size() > 1) {
-    const int en = eng->EnablePeerAccess(parts);
-    KV_CHECK_EQ(en, static_cast<int>(parts.size() * (parts.size() - 1)))
-        << "GPU peer access is not available between all participating devices";
+    eng->RequirePeerAccess(parts);
     eng->JoinStreams(parts);
   }
   if (e.gc_merged.is_none() || e.gc_merged.dev() != home) {
     e.gc_merged = NDArray(e.shape, Context::GPU(home), kFloat32);
   }
-  for (size_t i = 0; i < nsrc; ++i) eng->BeginRead(home, *e.gc_compressed[i].var());
-  eng->BeginWrite(home, *e.gc_merged.var());
   {
-    DeviceGuard g(home);
+    LaneOp op(home);
+    for (size_t i = 0; i < nsrc; ++i) op.Read(e.gc_compressed[i]);
+    op.Write(e.gc_merged);
     LaunchDequantizeSum2Bit(comp_ptrs.data(), static_cast<int>(nsrc),
-                            static_cast<float*>(e.gc_merged.data()), n, gc_threshold_,
-                            eng->Stream(home));
+                            static_cast<float*>(e.gc_merged.data()), n, gc_threshold_, op.stream());
+    eng->CountLaunch("dequantize_sum_2bit", n * 4 + nsrc * words * 4);
+    op.Issue();
   }
-  eng->CountLaunch("dequantize_sum_2bit", n * 4 + nsrc * words * 4);
-  const uint64_t seq = eng->Issue(home);
-  eng->MarkWrite(home, seq, e.gc_merged.var());
-  for (size_t i = 0; i < nsrc; ++i) eng->MarkRead(home, seq, e.gc_compressed[i].var());
   if (parts.size() > 1) eng->JoinStreams(parts);
   return e.gc_merged;
 }

@@ -84,21 +84,12 @@ std::shared_ptr<PackList> BuildPackList(std::vector<std::pair<NDArray, NDArray>>
 }
 
 void RunPackList(PackList& pl) {
-  Engine* eng = Engine::Get();
-  const int lane = pl.lane;
-  for (auto& pr : pl.pairs) {
-    eng->BeginRead(lane, *pr.first.var());
-    eng->BeginWrite(lane, *pr.second.var());
-  }
-  DeviceGuard g(pl.dev);
-  LaunchPackBulk(static_cast<const PackItem*>(pl.d_items), pl.n_items, pl.total_bytes, eng->Stream(lane),
+  LaneOp op(pl.lane);
+  for (auto& pr : pl.pairs) op.Read(pr.first).Write(pr.second);
+  LaunchPackBulk(static_cast<const PackItem*>(pl.d_items), pl.n_items, pl.total_bytes, op.stream(),
                  pl.host_io ? 32 : 0);
-  eng->CountLaunch("pack_bulk(tma)", 2 * pl.total_bytes);
-  const uint64_t seq = eng->Issue(lane);
-  for (auto& pr : pl.pairs) {
-    eng->MarkRead(lane, seq, pr.first.var());
-    eng->MarkWrite(lane, seq, pr.second.var());
-  }
+  Engine::Get()->CountLaunch("pack_bulk(tma)", 2 * pl.total_bytes);
+  op.Issue();
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -315,11 +306,7 @@ void KVStore::PrepareDense(std::vector<DenseOp>& ops, int opt_kind, bool allow_s
       for (auto& o : op.outs) if (o.on_gpu()) part_set.insert(o.dev());
     }
     P.parts.assign(part_set.begin(), part_set.end());
-    if (P.parts.size() > 1) {
-      int enabled = eng->EnablePeerAccess(P.parts);
-      KV_CHECK_EQ(enabled, static_cast<int>(P.parts.size() * (P.parts.size() - 1)))
-          << "GPU peer access is not available between all participating devices";
-    }
+    eng->RequirePeerAccess(P.parts);
     const char* hm = std::getenv("B200KV_HOST_MODE");
     if (hm != nullptr && (std::string(hm) == "in_tma" || std::string(hm) == "pipe")) {
       P.pack_in = BuildPackList(&P.stage_in);
@@ -344,12 +331,12 @@ void KVStore::RunPrepared(Prepared& P) {
     KV_CHECK(g != nullptr) << "the peer group was destroyed while a store still uses it";
     const int dev = g->dev();
     NcclComm comm = g->NcclCommunicator();
-    eng->BeginWrite(dev, *P.nccl_bucket.var());
-    DeviceGuard guard(dev);
+    LaneOp op(dev);
+    op.Write(P.nccl_bucket);
     Nccl::Get()->AllReduceSum(P.nccl_bucket.data(), P.nccl_bucket.data(), P.nccl_bucket.Size(), P.dtype, comm,
-                              eng->Stream(dev));
+                              op.stream());
     eng->CountLaunch("ncclAllReduce", P.nccl_bucket.ByteSize());
-    eng->MarkWrite(dev, eng->Issue(dev), P.nccl_bucket.var());
+    op.Issue();
   }
 
   // ---- optimizer bookkeeping: update counts first (Optimizer._update_count, optimizer.py:412-430)

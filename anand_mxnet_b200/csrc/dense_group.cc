@@ -62,15 +62,8 @@ void KVStore::PrepareDenseNccl(std::vector<DenseOp>& ops, int opt_kind, std::vec
     P.is_push = is_push;
     P.owners = {dev};
     P.parts = {dev};
-    if (is_push) {
-      P.nccl_bucket = NDArray({static_cast<int64_t>(elems[kv.first])}, Context::GPU(dev), kv.first);
-      // the padding between keys is summed too: keep it finite
-      DeviceGuard guard(dev);
-      Engine* eng = Engine::Get();
-      eng->BeginWrite(dev, *P.nccl_bucket.var());
-      KV_CUDA(cudaMemsetAsync(P.nccl_bucket.data(), 0, P.nccl_bucket.ByteSize(), eng->Stream(dev)));
-      eng->MarkWrite(dev, eng->Issue(dev), P.nccl_bucket.var());
-    }
+    // the padding between keys is summed too: keep it finite
+    if (is_push) P.nccl_bucket = ZerosOn({static_cast<int64_t>(elems[kv.first])}, dev, kv.first);
     size_t off = 0;
     for (auto& op : P.ops) {
       KeyEntry& e = *op.e;
@@ -104,19 +97,18 @@ void KVStore::PrepareDenseNccl(std::vector<DenseOp>& ops, int opt_kind, std::vec
 void KVStore::BroadcastInitNccl(const std::vector<int>& keys) {
   PeerGroup* g = PeerGroup::Get();
   const int dev = g->dev();
-  Engine* eng = Engine::Get();
   NcclComm comm = g->NcclCommunicator();
   DeviceGuard guard(dev);
-  cudaStream_t st = eng->Stream(dev);
   for (int key : keys) {
     KeyEntry& e = Entry(key);
     if (e.stype != kDefaultStorage) continue;
     if (e.home < 0) EnsureOnDevice(e, dev);
     KV_CHECK_EQ(e.home, dev) << "one-rank-per-GPU store: initialise keys on this rank's GPU";
     NDArray& w = e.dev[dev].w;
-    eng->BeginWrite(dev, *w.var());
-    Nccl::Get()->Broadcast(w.data(), w.data(), e.size, e.dtype, 0, comm, st);
-    eng->MarkWrite(dev, eng->Issue(dev), w.var());
+    LaneOp op(dev);
+    op.Write(w);
+    Nccl::Get()->Broadcast(w.data(), w.data(), e.size, e.dtype, 0, comm, op.stream());
+    op.Issue();
   }
 }
 

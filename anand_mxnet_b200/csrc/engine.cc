@@ -344,6 +344,12 @@ int Engine::EnablePeerAccess(const std::vector<int>& devs) {
   return enabled;
 }
 
+void Engine::RequirePeerAccess(const std::vector<int>& devs) {
+  if (devs.size() < 2) return;
+  KV_CHECK_EQ(EnablePeerAccess(devs), static_cast<int>(devs.size() * (devs.size() - 1)))
+      << "GPU peer access is not available between all participating devices";
+}
+
 bool Engine::PeerEnabled(int a, int b) { return a == b || peer_[a][b]; }
 
 void Engine::CountLaunch(const char* name, uint64_t algorithmic_bytes) {

@@ -59,6 +59,7 @@ class Engine {
 
   // ---- dependency protocol: call BeginRead/BeginWrite before enqueueing an op on lane `sid`, then
   // Issue(sid) once the op is enqueued and Mark* the arrays with the returned sequence number.
+  // An op on one lane uses LaneOp (ndarray.h), which names each array once for both steps.
   void BeginRead(int sid, const Var& v);   // lane waits for v's writer
   void BeginWrite(int sid, const Var& v);  // ... and for every reader
   uint64_t Issue(int sid);
@@ -97,6 +98,8 @@ class Engine {
 
   // src/kvstore/comm.h:715-757 (EnableP2P): returns the number of ordered pairs enabled
   int EnablePeerAccess(const std::vector<int>& devs);
+  // ... and fails unless every ordered pair of `devs` has peer access
+  void RequirePeerAccess(const std::vector<int>& devs);
   bool PeerEnabled(int a, int b);
 
   std::recursive_mutex& mutex() { return mu_; }

@@ -772,26 +772,13 @@ void KVStore::EnsureWhole(KeyEntry& e, int dev) {
   ++layout_epoch_;
 }
 
-static NDArray ZeroState(const KeyEntry& e, int dev) {
-  NDArray a(e.shape, Context::GPU(dev), kFloat32);
-  if (a.Size() == 0) return a;
-  Engine* eng = Engine::Get();
-  DeviceGuard g(dev);
-  // a recycled block carries the pending work of its previous owner (possibly on a copy lane or
-  // a peer GPU): the memset is the first writer and must wait for it
-  eng->BeginWrite(dev, *a.var());
-  KV_CUDA(cudaMemsetAsync(a.data(), 0, a.ByteSize(), eng->Stream(dev)));
-  eng->MarkWrite(dev, eng->Issue(dev), a.var());
-  return a;
-}
-
 DevState& KVStore::StateOn(KeyEntry& e, int dev, int opt_kind) {
   DevState& s = e.dev[dev];
   if (s.w.is_none()) s.w = NDArray(e.shape, Context::GPU(dev), e.dtype);
   if (opt_kind == kOptSGD || opt_kind == kOptAdam) {
     const bool need_s1 = opt_kind == kOptAdam || opt_.momentum != 0.0;  // SGD.create_state
-    if (need_s1 && s.s1.is_none()) s.s1 = ZeroState(e, dev);
-    if (opt_kind == kOptAdam && s.s2.is_none()) s.s2 = ZeroState(e, dev);
+    if (need_s1 && s.s1.is_none()) s.s1 = ZerosOn(e.shape, dev, kFloat32);
+    if (opt_kind == kOptAdam && s.s2.is_none()) s.s2 = ZerosOn(e.shape, dev, kFloat32);
     if (Is16Bit(e.dtype)) {
       KV_CHECK(opt_.multi_precision)
           << "16-bit key " << e.key << ": the fused optimizer keeps fp32 master weights; create "
@@ -799,14 +786,11 @@ DevState& KVStore::StateOn(KeyEntry& e, int dev, int opt_kind) {
       if (s.w32.is_none()) {
         // create_state_multi_precision: weight_master_copy = weight.astype(float32)
         s.w32 = NDArray(e.shape, Context::GPU(dev), kFloat32);
-        Engine* eng = Engine::Get();
-        eng->BeginRead(dev, *s.w.var());
-        DeviceGuard g(dev);
-        LaunchCast(s.w32.data(), kFloat32, s.w.data(), e.dtype, e.size, eng->Stream(dev));
-        eng->CountLaunch("cast", e.size * (4 + DTypeSize(e.dtype)));
-        uint64_t seq = eng->Issue(dev);
-        eng->MarkRead(dev, seq, s.w.var());
-        eng->MarkWrite(dev, seq, s.w32.var());
+        LaneOp op(dev);
+        op.Read(s.w).Write(s.w32);
+        LaunchCast(s.w32.data(), kFloat32, s.w.data(), e.dtype, e.size, op.stream());
+        Engine::Get()->CountLaunch("cast", e.size * (4 + DTypeSize(e.dtype)));
+        op.Issue();
       }
     }
   }

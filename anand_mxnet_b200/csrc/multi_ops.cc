@@ -100,15 +100,15 @@ struct Call {
 void Run(Call& c) {
   KV_CHECK(!c.tensors.empty());
   Engine* eng = Engine::Get();
-  DeviceGuard guard(c.dev);
-  cudaStream_t st = eng->Stream(c.dev);
+  LaneOp op(c.dev);
+  cudaStream_t st = op.stream();
   for (auto& a : c.reads) {
     KV_CHECK(a.on_gpu() && a.dev() == c.dev) << "all operands must be on the same GPU (no CPU fallback)";
-    eng->BeginRead(c.dev, *a.var());
+    op.Read(a);
   }
   for (auto& a : c.writes) {
     KV_CHECK(a.on_gpu() && a.dev() == c.dev) << "all operands must be on the same GPU (no CPU fallback)";
-    eng->BeginWrite(c.dev, *a.var());
+    op.Write(a);
   }
   for (size_t g0 = 0; g0 < c.tensors.size(); g0 += kMTMaxTensors) {
     const size_t g1 = std::min(c.tensors.size(), g0 + kMTMaxTensors);
@@ -135,9 +135,7 @@ void Run(Call& c) {
       eng->CountLaunch("multi_tensor_finalize", 0);
     }
   }
-  uint64_t seq = eng->Issue(c.dev);
-  for (auto& a : c.reads) eng->MarkRead(c.dev, seq, a.var());
-  for (auto& a : c.writes) eng->MarkWrite(c.dev, seq, a.var());
+  op.Issue();
 }
 
 MTTensor Tensor(std::initializer_list<const NDArray*> arrs, size_t size, uint32_t aux, int dtype) {
@@ -235,19 +233,14 @@ bool MultiTensorOp(const std::string& n, const std::vector<NDArray>& in, std::ve
     const float eta = Required(p, "eta", n), eps = Required(p, "eps", n);
     const float rescale = GetF(p, "rescale_grad", 1.0f);
     KV_CHECK(in[0].on_gpu()) << "multi_lars runs on GPU arrays only (no CPU fallback)";
-    const int dev = in[0].dev();
-    Engine* eng = Engine::Get();
-    DeviceGuard guard(dev);
-    for (int i = 0; i < 4; ++i) eng->BeginRead(dev, *in[i].var());
-    eng->BeginWrite(dev, *out.var());
+    LaneOp op(in[0].dev());
+    op.Read(in[0]).Read(in[1]).Read(in[2]).Read(in[3]).Write(out);
     LaunchMultiLars(static_cast<int>(cnt), static_cast<float*>(out.data()),
                     static_cast<const float*>(in[0].data()), static_cast<const float*>(in[1].data()),
                     static_cast<const float*>(in[2].data()), static_cast<const float*>(in[3].data()),
-                    eta, eps, rescale, eng->Stream(dev));
-    eng->CountLaunch("multi_lars", 0);
-    uint64_t seq = eng->Issue(dev);
-    for (int i = 0; i < 4; ++i) eng->MarkRead(dev, seq, in[i].var());
-    eng->MarkWrite(dev, seq, out.var());
+                    eta, eps, rescale, op.stream());
+    Engine::Get()->CountLaunch("multi_lars", 0);
+    op.Issue();
     return true;
   }
   // --------------------------------------------------------------------- adamw (single + multi)

@@ -211,18 +211,51 @@ void RawCopy(void* dst, Context dctx, Var* dvar, const void* src, Context sctx, 
   if (dctx.is_gpu() && sctx.is_gpu()) lane = dctx.dev_id;
   else if (dctx.is_gpu()) lane = Engine::CopyInLane(dctx.dev_id);
   else lane = Engine::CopyOutLane(sctx.dev_id);
-  cudaStream_t s = e->Stream(lane);
-  e->BeginRead(lane, *svar);
-  e->BeginWrite(lane, *dvar);
-  DeviceGuard g(Engine::DevOf(lane));
+  LaneOp op(lane);
+  op.Read(svar).Write(dvar);
   if (dctx.is_gpu() && sctx.is_gpu() && dctx.dev_id != sctx.dev_id) {
-    KV_CUDA(cudaMemcpyPeerAsync(dst, dctx.dev_id, src, sctx.dev_id, bytes, s));
+    KV_CUDA(cudaMemcpyPeerAsync(dst, dctx.dev_id, src, sctx.dev_id, bytes, op.stream()));
   } else {
-    KV_CUDA(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDefault, s));
+    KV_CUDA(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDefault, op.stream()));
   }
-  uint64_t seq = e->Issue(lane);
-  e->MarkRead(lane, seq, svar);
-  e->MarkWrite(lane, seq, dvar);
+  op.Issue();
+}
+
+LaneOp::LaneOp(int lane)
+    : lane_(lane), stream_(Engine::Get()->Stream(lane)), guard_(Engine::DevOf(lane)) {}
+
+LaneOp& LaneOp::Add(Var* v, bool write, const std::shared_ptr<Storage>& keep) {
+  Engine* e = Engine::Get();
+  if (write) e->BeginWrite(lane_, *v);
+  else e->BeginRead(lane_, *v);
+  if (n_ >= kInline) spill_.emplace_back();
+  Use& u = At(n_++);
+  u.var = v;
+  u.write = write;
+  u.keep = keep;
+  return *this;
+}
+
+uint64_t LaneOp::Issue() {
+  Engine* e = Engine::Get();
+  const uint64_t seq = e->Issue(lane_);
+  for (int i = 0; i < n_; ++i) {
+    if (!At(i).write) e->MarkRead(lane_, seq, At(i).var);
+  }
+  for (int i = 0; i < n_; ++i) {
+    if (At(i).write) e->MarkWrite(lane_, seq, At(i).var);
+  }
+  return seq;
+}
+
+NDArray ZerosOn(const std::vector<int64_t>& shape, int dev, int dtype) {
+  NDArray a(shape, Context::GPU(dev), dtype);
+  if (a.Size() == 0) return a;
+  LaneOp op(dev);
+  op.Write(a);
+  KV_CUDA(cudaMemsetAsync(a.data(), 0, a.ByteSize(), op.stream()));
+  op.Issue();
+  return a;
 }
 
 void CopyFromTo(const NDArray& from, const NDArray& to) {

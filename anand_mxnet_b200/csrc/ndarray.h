@@ -117,6 +117,7 @@ class NDArray {
   NDArray Copy(Context ctx) const;
 
  private:
+  friend class LaneOp;
   std::shared_ptr<Storage> st_;
   SharedShape shape_;
   int dtype_ = kFloat32;
@@ -132,5 +133,52 @@ void CopyFromTo(const NDArray& from, const NDArray& to);
 // host<->device staging of MXNDArraySyncCopy*.
 void RawCopy(void* dst, Context dctx, Var* dvar, const void* src, Context sctx, Var* svar,
              size_t bytes);
+
+// One operation on one engine lane (the reference's Engine::PushAsync with its const and mutable
+// var lists), with the lane's device current for its lifetime:
+//     LaneOp op(lane);
+//     op.Read(a).Write(b);   // the lane waits for a's writer, and for b's writer and readers
+//     ... enqueue on op.stream() ...
+//     op.Issue();            // marks a read and b written by this operation
+// Each array is named once, so its wait and its mark cannot disagree. Issue() marks the reads
+// before the writes: an array declared both ways ends as written. The declared arrays are held
+// until the op is destroyed, so scratch arrays outlive their marks. An op destroyed without Issue()
+// (an exception between declaring and enqueueing) marks nothing. A none array (an absent optional
+// operand) is skipped.
+class LaneOp {
+ public:
+  explicit LaneOp(int lane);
+  LaneOp(const LaneOp&) = delete;
+  LaneOp& operator=(const LaneOp&) = delete;
+
+  LaneOp& Read(const NDArray& a) { return a.is_none() ? *this : Add(a.var(), false, a.st_); }
+  LaneOp& Write(const NDArray& a) { return a.is_none() ? *this : Add(a.var(), true, a.st_); }
+  LaneOp& Read(Var* v) { return Add(v, false, nullptr); }   // the caller keeps *v alive
+  LaneOp& Write(Var* v) { return Add(v, true, nullptr); }
+  int lane() const { return lane_; }
+  cudaStream_t stream() const { return stream_; }
+  uint64_t Issue();  // returns the operation's sequence number on the lane
+
+ private:
+  struct Use {
+    Var* var = nullptr;
+    bool write = false;
+    std::shared_ptr<Storage> keep;
+  };
+  LaneOp& Add(Var* v, bool write, const std::shared_ptr<Storage>& keep);
+  Use& At(int i) { return i < kInline ? inline_[i] : spill_[i - kInline]; }
+
+  static constexpr int kInline = 8;  // no heap allocation for the common operation
+  int lane_;
+  cudaStream_t stream_;
+  DeviceGuard guard_;
+  Use inline_[kInline];
+  std::vector<Use> spill_;
+  int n_ = 0;
+};
+
+// A dense array of zeros on GPU `dev`, filled on that GPU's compute lane. The fill is the array's
+// first writer, so it waits for whatever a recycled block's previous owner left pending.
+NDArray ZerosOn(const std::vector<int64_t>& shape, int dev, int dtype);
 
 }  // namespace b200kv

@@ -108,8 +108,8 @@ void RunAdhoc(int opt, std::vector<AdhocKey>& keys, const DenseLaunch& scalars,
   auto& cache = PlanCache();
   std::shared_ptr<AdhocPlan> plan;
   auto it = cache.find(sig);
-  DeviceGuard guard(dev);
-  cudaStream_t st = eng->Stream(dev);
+  LaneOp op(dev);
+  cudaStream_t st = op.stream();
   if (it != cache.end()) {
     plan = it->second;
   } else {
@@ -157,13 +157,7 @@ void RunAdhoc(int opt, std::vector<AdhocKey>& keys, const DenseLaunch& scalars,
     hyper[2 * i + 1] = keys[i].wd;
   }
   KV_CUDA(cudaMemcpyAsync(plan->d_hyper, hyper.data(), plan->bh, cudaMemcpyHostToDevice, st));
-  for (auto& k : keys) {
-    if (!k.g.is_none()) eng->BeginRead(dev, *k.g.var());
-    eng->BeginWrite(dev, *k.w.var());
-    for (const NDArray* a : {&k.s1, &k.s2, &k.w32}) {
-      if (!a->is_none()) eng->BeginWrite(dev, *a->var());
-    }
-  }
+  for (auto& k : keys) op.Read(k.g).Write(k.w).Write(k.s1).Write(k.s2).Write(k.w32);
   DenseLaunch L = scalars;
   if (lrs != nullptr) {
     // preloaded_multi_*: per-tensor lr / wd are read from device arrays by the kernel
@@ -172,7 +166,7 @@ void RunAdhoc(int opt, std::vector<AdhocKey>& keys, const DenseLaunch& scalars,
       KV_CHECK_EQ(a->dtype(), kFloat32) << "lrs / wds must be float32";
       KV_CHECK_EQ(a->Size(), keys.size()) << "Number of learning rates / weight decays is "
                                           << "inconsistent with num_weights parameter passed";
-      eng->BeginRead(dev, *a->var());
+      op.Read(*a);
     }
     L.lrs = static_cast<const float*>(lrs->data());
     L.wds = static_cast<const float*>(wds->data());
@@ -186,18 +180,7 @@ void RunAdhoc(int opt, std::vector<AdhocKey>& keys, const DenseLaunch& scalars,
   L.opt = opt;
   LaunchDenseFused(L, st);
   eng->CountLaunch("dense_fused(op)", 0);
-  uint64_t seq = eng->Issue(dev);
-  for (auto& k : keys) {
-    if (!k.g.is_none()) eng->MarkRead(dev, seq, k.g.var());
-    eng->MarkWrite(dev, seq, k.w.var());
-    for (const NDArray* a : {&k.s1, &k.s2, &k.w32}) {
-      if (!a->is_none()) eng->MarkWrite(dev, seq, a->var());
-    }
-  }
-  if (lrs != nullptr) {
-    eng->MarkRead(dev, seq, lrs->var());
-    eng->MarkRead(dev, seq, wds->var());
-  }
+  op.Issue();
 }
 
 // lazy row_sparse gradient: update only the rows listed (optimizer_op-inl.h:452-565,803-876,1410-1470)
@@ -208,13 +191,8 @@ void RunRspUpdate(int opt, const NDArray& w, const NDArray& g, const NDArray& s1
   KV_CHECK_EQ(w.stype(), kDefaultStorage) << "row_sparse weights with row_sparse gradients: the "
                                           << "store keeps sparse-updated weights dense";
   if (!g.storage_initialized()) return;  // all-zero gradient: lazy update touches nothing
-  const int dev = w.dev();
-  Engine* eng = Engine::Get();
-  DeviceGuard guard(dev);
-  eng->BeginRead(dev, *g.var());
-  eng->BeginWrite(dev, *w.var());
-  if (!s1.is_none()) eng->BeginWrite(dev, *s1.var());
-  if (!s2.is_none()) eng->BeginWrite(dev, *s2.var());
+  LaneOp op(w.dev());
+  op.Read(g).Write(w).Write(s1).Write(s2);
   L.opt = opt;
   L.w = static_cast<float*>(w.data());
   L.s1 = s1.is_none() ? nullptr : static_cast<float*>(s1.data());
@@ -223,13 +201,9 @@ void RunRspUpdate(int opt, const NDArray& w, const NDArray& g, const NDArray& s1
   L.gval = static_cast<const float*>(g.data());
   L.nrows = g.nnr();
   L.row_len = static_cast<int64_t>(w.RowLength());
-  LaunchRspUpdate(L, eng->Stream(dev));
-  eng->CountLaunch("rsp_update", 0);
-  uint64_t seq = eng->Issue(dev);
-  eng->MarkRead(dev, seq, g.var());
-  eng->MarkWrite(dev, seq, w.var());
-  if (!s1.is_none()) eng->MarkWrite(dev, seq, s1.var());
-  if (!s2.is_none()) eng->MarkWrite(dev, seq, s2.var());
+  LaunchRspUpdate(L, op.stream());
+  Engine::Get()->CountLaunch("rsp_update", 0);
+  op.Issue();
 }
 
 NDArray OutOrInput(std::vector<NDArray>* outputs, size_t i, const NDArray& like) {
@@ -242,28 +216,24 @@ NDArray OutOrInput(std::vector<NDArray>* outputs, size_t i, const NDArray& like)
 void Elementwise(int op, const NDArray& a, const NDArray* b, float scalar, const NDArray& out) {
   KV_CHECK(out.on_gpu()) << "elementwise operators run on GPU arrays only";
   const int dev = out.dev();
-  Engine* eng = Engine::Get();
-  DeviceGuard guard(dev);
+  LaneOp lop(dev);
   if (op != kEwFill) {
     KV_CHECK(a.on_gpu() && a.dev() == dev) << "all operands must be on the same GPU";
     KV_CHECK_EQ(a.Size(), out.Size()) << "elementwise shape mismatch";
     KV_CHECK_EQ(a.dtype(), out.dtype()) << "elementwise dtype mismatch";
-    eng->BeginRead(dev, *a.var());
+    lop.Read(a);
   }
   if (b) {
     KV_CHECK(b->on_gpu() && b->dev() == dev) << "all operands must be on the same GPU";
     KV_CHECK_EQ(b->Size(), out.Size()) << "elementwise shape mismatch";
     KV_CHECK_EQ(b->dtype(), out.dtype()) << "elementwise dtype mismatch";
-    eng->BeginRead(dev, *b->var());
+    lop.Read(*b);
   }
-  eng->BeginWrite(dev, *out.var());
+  lop.Write(out);
   LaunchElementwise(op, out.dtype(), out.data(), op == kEwFill ? nullptr : a.data(),
-                    b ? b->data() : nullptr, scalar, out.Size(), eng->Stream(dev));
-  eng->CountLaunch("elementwise", 0);
-  uint64_t seq = eng->Issue(dev);
-  if (op != kEwFill) eng->MarkRead(dev, seq, a.var());
-  if (b) eng->MarkRead(dev, seq, b->var());
-  eng->MarkWrite(dev, seq, out.var());
+                    b ? b->data() : nullptr, scalar, out.Size(), lop.stream());
+  Engine::Get()->CountLaunch("elementwise", 0);
+  lop.Issue();
 }
 
 }  // namespace
@@ -451,16 +421,11 @@ void InvokeOp(const OpInfo* op, const std::vector<NDArray>& in, std::vector<NDAr
       o = (*outputs)[0];
     }
     KV_CHECK(in[0].on_gpu() && o.on_gpu() && in[0].dev() == o.dev()) << "cast runs on one GPU";
-    const int dev = o.dev();
-    Engine* eng = Engine::Get();
-    DeviceGuard guard(dev);
-    eng->BeginRead(dev, *in[0].var());
-    eng->BeginWrite(dev, *o.var());
-    LaunchCast(o.data(), o.dtype(), in[0].data(), in[0].dtype(), o.Size(), eng->Stream(dev));
-    eng->CountLaunch("cast", 0);
-    uint64_t seq = eng->Issue(dev);
-    eng->MarkRead(dev, seq, in[0].var());
-    eng->MarkWrite(dev, seq, o.var());
+    LaneOp op(o.dev());
+    op.Read(in[0]).Write(o);
+    LaunchCast(o.data(), o.dtype(), in[0].data(), in[0].dtype(), o.Size(), op.stream());
+    Engine::Get()->CountLaunch("cast", 0);
+    op.Issue();
     return;
   }
   KV_FATAL << "operator " << n << " is registered but not implemented";

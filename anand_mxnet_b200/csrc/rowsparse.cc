@@ -55,13 +55,54 @@ int BitsFor(int64_t n) {  // bits that hold every id in [0, n)
   return b;
 }
 
-struct Scratch {
-  int dev;
-  void* p;
-  size_t bytes;
-  Scratch(int d, size_t b) : dev(d), p(Engine::Get()->Alloc(d, b)), bytes(b) {}
-  ~Scratch() { Engine::Get()->Free(dev, p, bytes); }
-};
+// The union's inputs: the sources that hold rows, in the order given.
+RspSources LocalSources(const std::vector<NDArray>& srcs) {
+  RspSources S;
+  int64_t total = 0;
+  for (auto& s : srcs) {
+    if (!s.storage_initialized()) continue;  // all-zero source
+    S.idx[S.nsrc] = s.row_ids();
+    S.val[S.nsrc] = static_cast<const float*>(s.data());
+    S.start[S.nsrc] = total;
+    total += s.nnr();
+    ++S.nsrc;
+  }
+  S.start[S.nsrc] = total;
+  return S;
+}
+
+// One rank per GPU: the union's inputs are every rank's gradient, read through IPC in rank order
+// (the reference's value-list order). `*src` becomes this rank's gradient, copied into the IPC arena
+// when the peers cannot address it where it is. Addresses and row counts change every step, so
+// they travel by a host all-gather on every push.
+RspSources RankSources(PeerGroup* g, int64_t key, const NDArray& src_in, NDArray* src) {
+  *src = src_in;
+  if (!src->on_gpu() || src->dev() != g->dev() ||
+      (src->storage_initialized() && !(g->InArena(src->data()) && g->InArena(src->row_ids())))) {
+    *src = src_in.Copy(Context::GPU(g->dev()));
+  }
+  const int64_t my_nnr = src->storage_initialized() ? src->nnr() : 0;
+  if (my_nnr > 0) {
+    KV_CHECK(g->InArena(src->data()) && g->InArena(src->row_ids()))
+        << "IPC arena exhausted; raise B200KV_IPC_ARENA_MB";
+  }
+  const std::vector<int64_t> all = g->AllGatherI64(
+      {my_nnr > 0 ? g->OffsetOf(src->row_ids()) : 0, my_nnr > 0 ? g->OffsetOf(src->data()) : 0, my_nnr, key});
+  RspSources S;
+  int64_t total = 0;
+  for (int r = 0; r < g->world(); ++r) {
+    KV_CHECK_EQ(all[4 * r + 3], key) << "one-rank-per-GPU store: rank " << r << " pushed a different row_sparse key";
+    const int64_t n = all[4 * r + 2];
+    if (n == 0) continue;
+    S.idx[S.nsrc] = static_cast<const int64_t*>(g->PeerPtr(r, all[4 * r]));
+    S.val[S.nsrc] = static_cast<const float*>(g->PeerPtr(r, all[4 * r + 1]));
+    S.start[S.nsrc] = total;
+    total += n;
+    ++S.nsrc;
+  }
+  S.start[S.nsrc] = total;
+  return S;
+}
 
 }  // namespace
 
@@ -93,23 +134,10 @@ void KVStore::PushRowSparse(KeyEntry& e, const std::vector<NDArray>& srcs_in) {
       if (std::find(parts.begin(), parts.end(), s.dev()) == parts.end()) parts.push_back(s.dev());
     }
   }
-  if (parts.size() > 1) {
-    int en = eng->EnablePeerAccess(parts);
-    KV_CHECK_EQ(en, static_cast<int>(parts.size() * (parts.size() - 1)))
-        << "GPU peer access is not available between all participating devices";
-  }
+  eng->RequirePeerAccess(parts);
   // ---- union of ids + ordered sum, all on the owner's stream, row count left on the device
-  RspSources S;
-  int64_t total = 0;
-  for (auto& s : srcs) {
-    if (!s.storage_initialized()) continue;  // all-zero source
-    S.idx[S.nsrc] = s.row_ids();
-    S.val[S.nsrc] = static_cast<const float*>(s.data());
-    S.start[S.nsrc] = total;
-    total += s.nnr();
-    ++S.nsrc;
-  }
-  S.start[S.nsrc] = total;
+  const RspSources S = LocalSources(srcs);
+  int64_t total = S.start[S.nsrc];
   NDArray merged = NDArray::RowSparse(e.shape, Context::GPU(home), e.dtype);
   const int64_t row_len = static_cast<int64_t>(e.rsp.RowLength());
   const bool on_store = opt_.enabled && (opt_.kind == kOptSGD || opt_.kind == kOptAdam);
@@ -132,15 +160,9 @@ void KVStore::PushRowSparse(KeyEntry& e, const std::vector<NDArray>& srcs_in) {
     double lrd = opt_.lr * (lm == opt_.lr_mult.end() ? 1.0 : lm->second);
     double wdd = opt_.wd * (wm == opt_.wd_mult.end() ? 1.0 : wm->second);
     DevState& s = e.dev[home];
-    const std::vector<int64_t> dshape = e.shape;
     const bool sharded_now = !e.rsp_devs.empty() || e.rsp_group || (dist_ && fused);   // state lives with the shards
     auto zero_state = [&](NDArray* a) {
-      if (!a->is_none() || sharded_now) return;
-      *a = NDArray(dshape, Context::GPU(home), kFloat32);
-      DeviceGuard g(home);
-      eng->BeginWrite(home, *a->var());   // first writer of a possibly recycled block
-      KV_CUDA(cudaMemsetAsync(a->data(), 0, a->ByteSize(), eng->Stream(home)));
-      eng->MarkWrite(home, eng->Issue(home), a->var());
+      if (a->is_none() && !sharded_now) *a = ZerosOn(e.shape, home, kFloat32);
     };
     if (opt_.kind == kOptSGD) {
       U.opt = opt_.momentum != 0.0 ? kOptSGD : kOptSGDSingle;  // sgd_mom_update / sgd_update
@@ -188,41 +210,32 @@ void KVStore::PushRowSparse(KeyEntry& e, const std::vector<NDArray>& srcs_in) {
     U.s2 = hs.s2.is_none() ? nullptr : static_cast<float*>(hs.s2.data());
   }
   if (total > 0) {
+    const int bits = BitsFor(e.shape[0]);
     NDArray d_nnr({1}, Context::GPU(home), kInt64);
+    NDArray ws({static_cast<int64_t>(RspMergeWorkspaceBytes(total, bits, S.nsrc))}, Context::GPU(home), kUint8);
     // fused: the summed rows are consumed in registers by the optimizer step, nothing is stored
     if (!fused) merged.CheckAndAllocRows(total);  // upper bound; nnr is set once the count is known
+    // the sources are read on their own lanes; the joins order those lanes around the home lane's work
     for (auto& s : srcs) eng->BeginRead(s.dev(), *s.var());
-    if (fused) {
-      eng->BeginWrite(home, *e.rsp.var());
-      DevState& ds = e.dev[home];
-      if (!ds.s1.is_none()) eng->BeginWrite(home, *ds.s1.var());
-      if (!ds.s2.is_none()) eng->BeginWrite(home, *ds.s2.var());
-    }
+    LaneOp op(home);
+    if (fused) op.Write(e.rsp).Write(e.dev[home].s1).Write(e.dev[home].s2);
+    else op.Write(merged);
+    op.Write(d_nnr).Write(ws);
     if (parts.size() > 1) eng->JoinStreams(parts);
-    DeviceGuard g(home);
-    cudaStream_t st = eng->Stream(home);
-    Scratch ws(home, RspMergeWorkspaceBytes(total, BitsFor(e.shape[0]), S.nsrc));
-    LaunchRspMerge(S, BitsFor(e.shape[0]), row_len, fused ? nullptr : merged.row_ids(),
+    LaunchRspMerge(S, bits, row_len, fused ? nullptr : merged.row_ids(),
                    fused ? nullptr : static_cast<float*>(merged.data()),
-                   static_cast<int64_t*>(d_nnr.data()), ws.p, ws.bytes, st, fused ? &U : nullptr);
+                   static_cast<int64_t*>(d_nnr.data()), ws.data(), ws.ByteSize(), op.stream(), fused ? &U : nullptr);
     eng->CountLaunch("rsp_merge(tag, sort, heads)", total * 24);
     eng->CountLaunch(fused ? "rsp_sum+update" : "rsp_sum", static_cast<uint64_t>(total) * row_len * 4 * 2);
     if (parts.size() > 1) eng->JoinStreams(parts);
-    uint64_t seq = eng->Issue(home);
-    eng->MarkWrite(home, seq, fused ? e.rsp.var() : merged.var());
-    eng->MarkWrite(home, seq, d_nnr.var());
-    if (fused) {
-      DevState& ds = e.dev[home];
-      if (!ds.s1.is_none()) eng->MarkWrite(home, seq, ds.s1.var());
-      if (!ds.s2.is_none()) eng->MarkWrite(home, seq, ds.s2.var());
-    }
+    const uint64_t seq = op.Issue();
     for (auto& s : srcs) {
       uint64_t sq = s.dev() == home ? seq : eng->Issue(s.dev());
       eng->MarkRead(s.dev(), sq, s.var());
     }
     if (!fused) {
       CountFence f(home, 1);
-      f.Post(static_cast<const int64_t*>(d_nnr.data()), st);
+      f.Post(static_cast<const int64_t*>(d_nnr.data()), op.stream());
       merged.SetNnr(f.Wait()[0]);
     }
   }
@@ -349,52 +362,34 @@ std::function<void()> KVStore::PullRowSparseGroup(int home, const std::vector<si
     total += n;
     id_bits = std::max(id_bits, BitsFor(e.shape[0]));
   }
-  if (parts.size() > 1) {
-    int en = eng->EnablePeerAccess(parts);
-    KV_CHECK_EQ(en, static_cast<int>(parts.size() * (parts.size() - 1)))
-        << "GPU peer access is not available between all participating devices";
-  }
-  // every dependency is taken on the lane that runs the kernels (`home`): arrays on other GPUs are
-  // reached through peer access, their writers / readers are waited for by events -- no stream
-  // join, so groups that run on different GPUs do not serialise each other
-  for (int k = 0; k < nitems; ++k) {
-    eng->BeginRead(home, *ids[k].var());
-    KeyEntry& ek = Entry(keys[which[k]]);
-    if (ek.rsp_devs.empty() && !ek.rsp_group) {
-      eng->BeginRead(home, *ek.rsp.var());
-    } else {
-      for (auto& sh : ek.rsp_shards) eng->BeginRead(home, *sh.var());
-    }
-    eng->BeginWrite(home, *targets[k].var());
-  }
+  eng->RequirePeerAccess(parts);
   auto fence = std::make_shared<CountFence>(home, nitems + 1);
   NDArray d_off({nitems + 1}, Context::GPU(home), kInt64);
   NDArray ws({static_cast<int64_t>(RetainBatchWorkspaceBytes(nitems, total, id_bits))}, Context::GPU(home), kUint8);
-  {
-    DeviceGuard g(home);
-    cudaStream_t st = eng->Stream(home);
-    LaunchUniqueBatch(items.data(), nitems, total, id_bits, static_cast<int64_t*>(d_off.data()),
-                      ws.data(), ws.ByteSize(), st);
-    eng->CountLaunch("unique_batch(gather, sort, unique, bounds)", total * 32);
-    fence->Post(static_cast<const int64_t*>(d_off.data()), st);
-    LaunchRetainBatch(nitems, total, id_bits, static_cast<const int64_t*>(d_off.data()), ws.data(), st);
-    uint64_t bytes = 0;
-    for (auto& it : items) bytes += static_cast<uint64_t>(it.n) * (it.row_len * 8 + 16);
-    eng->CountLaunch("sparse_retain", bytes);
-  }
-  uint64_t seq = eng->Issue(home);
-  eng->MarkWrite(home, seq, d_off.var());
-  eng->MarkWrite(home, seq, ws.var());
+  // every dependency is taken on the lane that runs the kernels (`home`): arrays on other GPUs are
+  // reached through peer access, their writers / readers are waited for by events -- no stream
+  // join, so groups that run on different GPUs do not serialise each other
+  LaneOp op(home);
   for (int k = 0; k < nitems; ++k) {
     KeyEntry& ek = Entry(keys[which[k]]);
+    op.Read(ids[k]);
     if (ek.rsp_devs.empty() && !ek.rsp_group) {
-      eng->MarkRead(home, seq, ek.rsp.var());
+      op.Read(ek.rsp);
     } else {
-      for (auto& sh : ek.rsp_shards) eng->MarkRead(home, seq, sh.var());
+      for (auto& sh : ek.rsp_shards) op.Read(sh);
     }
-    eng->MarkRead(home, seq, ids[k].var());
-    eng->MarkWrite(home, seq, targets[k].var());
+    op.Write(targets[k]);
   }
+  op.Write(d_off).Write(ws);
+  LaunchUniqueBatch(items.data(), nitems, total, id_bits, static_cast<int64_t*>(d_off.data()),
+                    ws.data(), ws.ByteSize(), op.stream());
+  eng->CountLaunch("unique_batch(gather, sort, unique, bounds)", total * 32);
+  fence->Post(static_cast<const int64_t*>(d_off.data()), op.stream());
+  LaunchRetainBatch(nitems, total, id_bits, static_cast<const int64_t*>(d_off.data()), ws.data(), op.stream());
+  uint64_t bytes = 0;
+  for (auto& it : items) bytes += static_cast<uint64_t>(it.n) * (it.row_len * 8 + 16);
+  eng->CountLaunch("sparse_retain", bytes);
+  op.Issue();
   // the counts are awaited by the caller AFTER every group of the call has been launched
   std::vector<NDArray> outs_k(nitems);
   for (int k = 0; k < nitems; ++k) outs_k[k] = outs[which[k]];
@@ -421,14 +416,9 @@ void RunRspStdUpdate(const NDArray& w, const NDArray& g, const NDArray& s1, cons
     // CheckAllRowsPresent (optimizer_op-inl.h:532-536)
     KV_CHECK_EQ(w.nnr(), rows) << "standard sparse update: the row_sparse weight must hold every row";
   }
-  Engine* eng = Engine::Get();
-  DeviceGuard guard(dev);
+  LaneOp op(dev);
   NDArray row_map({rows}, Context::GPU(dev), kInt32);
-  eng->BeginRead(dev, *g.var());
-  eng->BeginWrite(dev, *w.var());
-  eng->BeginWrite(dev, *row_map.var());
-  if (!s1.is_none()) eng->BeginWrite(dev, *s1.var());
-  if (!s2.is_none()) eng->BeginWrite(dev, *s2.var());
+  op.Read(g).Write(w).Write(row_map).Write(s1).Write(s2);
   L.w = static_cast<float*>(w.data());
   L.s1 = s1.is_none() ? nullptr : static_cast<float*>(s1.data());
   L.s2 = s2.is_none() ? nullptr : static_cast<float*>(s2.data());
@@ -437,14 +427,9 @@ void RunRspStdUpdate(const NDArray& w, const NDArray& g, const NDArray& s1, cons
   L.nrows = g.nnr();
   L.d_nrows = nullptr;
   L.row_len = static_cast<int64_t>(w.RowLength());
-  LaunchRspStdUpdate(L, rows, static_cast<int32_t*>(row_map.data()), eng->Stream(dev));
-  eng->CountLaunch("rsp_std_update", static_cast<uint64_t>(rows) * L.row_len * 8);
-  uint64_t seq = eng->Issue(dev);
-  eng->MarkRead(dev, seq, g.var());
-  eng->MarkWrite(dev, seq, w.var());
-  eng->MarkWrite(dev, seq, row_map.var());
-  if (!s1.is_none()) eng->MarkWrite(dev, seq, s1.var());
-  if (!s2.is_none()) eng->MarkWrite(dev, seq, s2.var());
+  LaunchRspStdUpdate(L, rows, static_cast<int32_t*>(row_map.data()), op.stream());
+  Engine::Get()->CountLaunch("rsp_std_update", static_cast<uint64_t>(rows) * L.row_len * 8);
+  op.Issue();
 }
 
 void CastStorageCopy(const NDArray& from_in, const NDArray& to) {
@@ -463,17 +448,15 @@ void CastStorageCopy(const NDArray& from_in, const NDArray& to) {
   if (to.stype() == kDefaultStorage) {
     // row_sparse -> dense (CastStorageRspDnsImpl): zeros, then the stored rows
     NDArray target = to.on_gpu() && to.dev() == dev ? to : NDArray(to.shape(), Context::GPU(dev), to.dtype());
-    eng->BeginRead(dev, *from.var());
-    eng->BeginWrite(dev, *target.var());
+    LaneOp op(dev);
+    op.Read(from).Write(target);
     KV_CUDA(cudaMemsetAsync(target.data(), 0, target.ByteSize(), st));
     if (from.storage_initialized()) {
       LaunchRspScatterRows(from.row_ids(), static_cast<const float*>(from.data()), from.nnr(), row_len,
                            static_cast<float*>(target.data()), st);
     }
     eng->CountLaunch("cast_storage(rsp->dns)", target.ByteSize());
-    uint64_t seq = eng->Issue(dev);
-    eng->MarkRead(dev, seq, from.var());
-    eng->MarkWrite(dev, seq, target.var());
+    op.Issue();
     if (!target.SameStorage(to)) CopyFromTo(target, to);
     return;
   }
@@ -487,15 +470,15 @@ void CastStorageCopy(const NDArray& from_in, const NDArray& to) {
   NDArray ids({rows}, Context::GPU(dev), kInt64);
   NDArray cnt({1}, Context::GPU(dev), kInt64);
   NDArray ws({static_cast<int64_t>(NonzeroRowsWorkspaceBytes(rows))}, Context::GPU(dev), kUint8);
-  eng->BeginRead(dev, *from.var());
-  for (const NDArray* a : {&ids, &cnt, &ws}) eng->BeginWrite(dev, *a->var());
-  LaunchNonzeroRows(static_cast<const float*>(from.data()), rows, row_len,
-                    static_cast<int64_t*>(ids.data()), static_cast<int64_t*>(cnt.data()), ws.data(),
-                    ws.ByteSize(), st);
-  eng->CountLaunch("cast_storage(nonzero rows)", from.ByteSize());
-  uint64_t seq = eng->Issue(dev);
-  eng->MarkRead(dev, seq, from.var());
-  for (const NDArray* a : {&ids, &cnt, &ws}) eng->MarkWrite(dev, seq, a->var());
+  {
+    LaneOp op(dev);
+    op.Read(from).Write(ids).Write(cnt).Write(ws);
+    LaunchNonzeroRows(static_cast<const float*>(from.data()), rows, row_len,
+                      static_cast<int64_t*>(ids.data()), static_cast<int64_t*>(cnt.data()), ws.data(),
+                      ws.ByteSize(), st);
+    eng->CountLaunch("cast_storage(nonzero rows)", from.ByteSize());
+    op.Issue();
+  }
   CountFence f(dev, 1);
   f.Post(static_cast<const int64_t*>(cnt.data()), st);
   const int64_t nnr = f.Wait()[0];
@@ -520,20 +503,12 @@ void CastStorageCopy(const NDArray& from_in, const NDArray& to) {
     NDArray off({2}, Context::GPU(dev), kInt64);
     const int id_bits = BitsFor(rows);
     NDArray rws({static_cast<int64_t>(RetainBatchWorkspaceBytes(1, nnr, id_bits))}, Context::GPU(dev), kUint8);
-    eng->BeginRead(dev, *from.var());
-    eng->BeginRead(dev, *ids.var());
-    eng->BeginWrite(dev, *target.var());
-    eng->BeginWrite(dev, *off.var());
-    eng->BeginWrite(dev, *rws.var());
+    LaneOp op(dev);
+    op.Read(from).Read(ids).Write(target).Write(off).Write(rws);
     LaunchUniqueBatch(&it, 1, nnr, id_bits, static_cast<int64_t*>(off.data()), rws.data(), rws.ByteSize(), st);
     LaunchRetainBatch(1, nnr, id_bits, static_cast<const int64_t*>(off.data()), rws.data(), st);
     eng->CountLaunch("cast_storage(dns->rsp gather)", static_cast<uint64_t>(nnr) * row_len * 8);
-    uint64_t sq = eng->Issue(dev);
-    eng->MarkRead(dev, sq, from.var());
-    eng->MarkRead(dev, sq, ids.var());
-    eng->MarkWrite(dev, sq, target.var());
-    eng->MarkWrite(dev, sq, off.var());
-    eng->MarkWrite(dev, sq, rws.var());
+    op.Issue();
   }
   if (!target.SameStorage(to)) CopyFromTo(target, to);
 }
@@ -651,74 +626,45 @@ bool KVStore::PushRowSparseSharded(KeyEntry& e, const std::vector<NDArray>& srcs
   const std::vector<int>& devs = e.rsp_devs;
   const int n = static_cast<int>(devs.size());
   const int64_t row_len = static_cast<int64_t>(e.rsp_shards[0].RowLength());
-  RspSources S;
-  int64_t total = 0;
-  for (auto& s : srcs) {
-    if (!s.storage_initialized()) continue;
-    S.idx[S.nsrc] = s.row_ids();
-    S.val[S.nsrc] = static_cast<const float*>(s.data());
-    S.start[S.nsrc] = total;
-    total += s.nnr();
-    ++S.nsrc;
-  }
-  S.start[S.nsrc] = total;
+  const RspSources S = LocalSources(srcs);
+  const int64_t total = S.start[S.nsrc];
   std::vector<int> lanes = devs;
   for (auto& s : srcs) {
     if (std::find(lanes.begin(), lanes.end(), s.dev()) == lanes.end()) lanes.push_back(s.dev());
   }
-  {
-    int en = eng->EnablePeerAccess(lanes);
-    KV_CHECK_EQ(en, static_cast<int>(lanes.size() * (lanes.size() - 1)))
-        << "GPU peer access is not available between all participating devices";
-  }
+  eng->RequirePeerAccess(lanes);
   // optimizer state of a shard is created on first use (zeros), like Optimizer.create_state
   const bool need1 = U.opt == kOptSGD || U.opt == kOptAdam, need2 = U.opt == kOptAdam;
   for (int j = 0; j < n; ++j) {
-    for (int which = 0; which < 2; ++which) {
-      NDArray& a = which == 0 ? e.rsp_shard_state[j].s1 : e.rsp_shard_state[j].s2;
-      if (!(which == 0 ? need1 : need2) || !a.is_none()) continue;
-      a = NDArray(e.rsp_shards[j].shape(), Context::GPU(devs[j]), kFloat32);
-      DeviceGuard g(devs[j]);
-      eng->BeginWrite(devs[j], *a.var());   // first writer of a possibly recycled block
-      KV_CUDA(cudaMemsetAsync(a.data(), 0, a.ByteSize(), eng->Stream(devs[j])));
-      eng->MarkWrite(devs[j], eng->Issue(devs[j]), a.var());
-    }
-  }
-  // each shard's kernels depend on the sources through events on ITS lane (no global join: the
-  // GPUs merge their row ranges concurrently and independently)
-  for (int j = 0; j < n; ++j) {
-    for (auto& s : srcs) eng->BeginRead(devs[j], *s.var());
-    eng->BeginWrite(devs[j], *e.rsp_shards[j].var());
-    if (need1) eng->BeginWrite(devs[j], *e.rsp_shard_state[j].s1.var());
-    if (need2) eng->BeginWrite(devs[j], *e.rsp_shard_state[j].s2.var());
+    DevState& sj = e.rsp_shard_state[j];
+    if (need1 && sj.s1.is_none()) sj.s1 = ZerosOn(e.rsp_shards[j].shape(), devs[j], kFloat32);
+    if (need2 && sj.s2.is_none()) sj.s2 = ZerosOn(e.rsp_shards[j].shape(), devs[j], kFloat32);
   }
   const int id_bits = BitsFor(rows);
-  std::vector<NDArray> keep;   // per-device scratch: lives until the kernels retire
   for (int j = 0; j < n; ++j) {
     const int64_t lo = static_cast<int64_t>(j) * e.rsp_rows_per, hi = std::min<int64_t>(rows, lo + e.rsp_rows_per);
     if (hi <= lo) continue;
     const int dev = devs[j];
-    DeviceGuard g(dev);
+    DevState& sj = e.rsp_shard_state[j];
     NDArray d_nnr({1}, Context::GPU(dev), kInt64);
     NDArray ws({static_cast<int64_t>(RspMergeWorkspaceBytes(total, id_bits, S.nsrc, lo, hi))}, Context::GPU(dev), kUint8);
+    // each shard's kernels depend on the sources through events on ITS lane (no global join: the
+    // GPUs merge their row ranges concurrently and independently)
+    LaneOp op(dev);
+    for (auto& s : srcs) op.Read(s);
+    op.Write(e.rsp_shards[j]).Write(d_nnr).Write(ws);
+    if (need1) op.Write(sj.s1);
+    if (need2) op.Write(sj.s2);
     RspUpdateLaunch Uj = U;
     // virtual bases: row `id` of the table is at base + id*row_len
     Uj.w = static_cast<float*>(e.rsp_shards[j].data()) - lo * row_len;
-    Uj.s1 = need1 ? static_cast<float*>(e.rsp_shard_state[j].s1.data()) - lo * row_len : nullptr;
-    Uj.s2 = need2 ? static_cast<float*>(e.rsp_shard_state[j].s2.data()) - lo * row_len : nullptr;
+    Uj.s1 = need1 ? static_cast<float*>(sj.s1.data()) - lo * row_len : nullptr;
+    Uj.s2 = need2 ? static_cast<float*>(sj.s2.data()) - lo * row_len : nullptr;
     LaunchRspMerge(S, id_bits, row_len, nullptr, nullptr, static_cast<int64_t*>(d_nnr.data()), ws.data(),
-                   ws.ByteSize(), eng->Stream(dev), &Uj, lo, hi);
+                   ws.ByteSize(), op.stream(), &Uj, lo, hi);
     eng->CountLaunch("rsp_merge(shard)", total * 24);
     eng->CountLaunch("rsp_sum+update(shard)", 0);
-    const uint64_t seq = eng->Issue(dev);
-    eng->MarkWrite(dev, seq, e.rsp_shards[j].var());
-    if (need1) eng->MarkWrite(dev, seq, e.rsp_shard_state[j].s1.var());
-    if (need2) eng->MarkWrite(dev, seq, e.rsp_shard_state[j].s2.var());
-    eng->MarkWrite(dev, seq, d_nnr.var());
-    eng->MarkWrite(dev, seq, ws.var());
-    for (auto& s : srcs) eng->MarkRead(dev, seq, s.var());
-    keep.push_back(d_nnr);
-    keep.push_back(ws);
+    op.Issue();
   }
   return true;
 }
@@ -748,61 +694,36 @@ NDArray KVStore::MergeRowSparseGroup(KeyEntry& e, const NDArray& src_in) {
   PeerGroup* g = PeerGroup::Get();
   KV_CHECK(g != nullptr);
   Engine* eng = Engine::Get();
-  const int dev = g->dev(), W = g->world();
+  const int dev = g->dev();
   KV_CHECK(!e.rsp_group) << "key " << e.key << " is sharded over the ranks by a fused optimizer; it "
                          << "cannot go back to a replicated value";
-  NDArray src = src_in;
-  if (!src.on_gpu() || src.dev() != dev ||
-      (src.storage_initialized() && !(g->InArena(src.data()) && g->InArena(src.row_ids())))) {
-    src = src_in.Copy(Context::GPU(dev));
-  }
-  const int64_t my_nnr = src.storage_initialized() ? src.nnr() : 0;
-  if (my_nnr > 0) {
-    KV_CHECK(g->InArena(src.data()) && g->InArena(src.row_ids()))
-        << "IPC arena exhausted; raise B200KV_IPC_ARENA_MB";
-  }
-  const std::vector<int64_t> all = g->AllGatherI64(
-      {my_nnr > 0 ? g->OffsetOf(src.row_ids()) : 0, my_nnr > 0 ? g->OffsetOf(src.data()) : 0, my_nnr,
-       static_cast<int64_t>(e.key)});
-  RspSources S;
-  int64_t total = 0;
-  for (int r = 0; r < W; ++r) {
-    KV_CHECK_EQ(all[4 * r + 3], static_cast<int64_t>(e.key))
-        << "one-rank-per-GPU store: rank " << r << " pushed a different row_sparse key";
-    const int64_t n = all[4 * r + 2];
-    if (n == 0) continue;
-    S.idx[S.nsrc] = static_cast<const int64_t*>(g->PeerPtr(r, all[4 * r]));
-    S.val[S.nsrc] = static_cast<const float*>(g->PeerPtr(r, all[4 * r + 1]));
-    S.start[S.nsrc] = total;
-    total += n;
-    ++S.nsrc;
-  }
-  S.start[S.nsrc] = total;
+  NDArray src;
+  const RspSources S = RankSources(g, e.key, src_in, &src);
+  const int64_t total = S.start[S.nsrc];
   NDArray merged = NDArray::RowSparse(e.shape, Context::GPU(dev), e.dtype);
   const int64_t row_len = static_cast<int64_t>(src.RowLength());
-  eng->BeginRead(dev, *src.var());
-  GroupBarrier();   // every rank's gradient is complete before anybody reads it
+  const int bits = BitsFor(e.shape[0]);
   NDArray d_nnr, ws;
   if (total > 0) {
-    DeviceGuard gd(dev);
     merged.CheckAndAllocRows(total);
     d_nnr = NDArray({1}, Context::GPU(dev), kInt64);
-    const int bits = BitsFor(e.shape[0]);
     ws = NDArray({static_cast<int64_t>(RspMergeWorkspaceBytes(total, bits, S.nsrc))}, Context::GPU(dev), kUint8);
+  }
+  // every wait is declared before the first barrier: none lands between the two
+  LaneOp op(dev);
+  op.Read(src).Write(merged).Write(d_nnr).Write(ws);
+  GroupBarrier();   // every rank's gradient is complete before anybody reads it
+  if (total > 0) {
     LaunchRspMerge(S, bits, row_len, merged.row_ids(), static_cast<float*>(merged.data()),
-                   static_cast<int64_t*>(d_nnr.data()), ws.data(), ws.ByteSize(), eng->Stream(dev));
+                   static_cast<int64_t*>(d_nnr.data()), ws.data(), ws.ByteSize(), op.stream());
     eng->CountLaunch("rsp_merge(replicated)", total * 24);
     eng->CountLaunch("rsp_sum(replicated)", static_cast<uint64_t>(total) * row_len * 8);
   }
   GroupBarrier();   // everybody has read the peers' gradients: they may be reused
-  const uint64_t seq = eng->Issue(dev);
-  eng->MarkRead(dev, seq, src.var());
-  eng->MarkWrite(dev, seq, merged.var());
+  op.Issue();
   if (total > 0) {
-    eng->MarkWrite(dev, seq, d_nnr.var());
-    eng->MarkWrite(dev, seq, ws.var());
     CountFence f(dev, 1);
-    f.Post(static_cast<const int64_t*>(d_nnr.data()), eng->Stream(dev));
+    f.Post(static_cast<const int64_t*>(d_nnr.data()), op.stream());
     merged.SetNnr(f.Wait()[0]);
   }
   return merged;
@@ -846,82 +767,44 @@ void KVStore::PushRowSparseGroup(KeyEntry& e, const NDArray& src_in, RspUpdateLa
   }
   const int64_t row_len = static_cast<int64_t>(e.rsp_shards[0].RowLength());
   const int64_t lo = R * e.rsp_rows_per, hi = std::min<int64_t>(rows, lo + e.rsp_rows_per);
-  // ---- the gradient must be addressable by the peers: inside this rank's arena
-  NDArray src = src_in;
-  if (!src.on_gpu() || src.dev() != dev ||
-      (src.storage_initialized() && !(g->InArena(src.data()) && g->InArena(src.row_ids())))) {
-    src = src_in.Copy(Context::GPU(dev));
-  }
-  const int64_t my_nnr = src.storage_initialized() ? src.nnr() : 0;
-  if (my_nnr > 0) {
-    KV_CHECK(g->InArena(src.data()) && g->InArena(src.row_ids()))
-        << "IPC arena exhausted; raise B200KV_IPC_ARENA_MB";
-  }
-  // per push: where every rank's gradient lives and how many rows it has (host all-gather: the
-  // arrays and row counts change every step)
-  const std::vector<int64_t> all = g->AllGatherI64(
-      {my_nnr > 0 ? g->OffsetOf(src.row_ids()) : 0, my_nnr > 0 ? g->OffsetOf(src.data()) : 0, my_nnr,
-       static_cast<int64_t>(e.key)});
-  RspSources S;
-  int64_t total = 0;
-  for (int r = 0; r < W; ++r) {            // rank order == the reference's value-list order
-    KV_CHECK_EQ(all[4 * r + 3], static_cast<int64_t>(e.key))
-        << "one-rank-per-GPU store: rank " << r << " pushed a different row_sparse key";
-    const int64_t n = all[4 * r + 2];
-    if (n == 0) continue;
-    S.idx[S.nsrc] = static_cast<const int64_t*>(g->PeerPtr(r, all[4 * r]));
-    S.val[S.nsrc] = static_cast<const float*>(g->PeerPtr(r, all[4 * r + 1]));
-    S.start[S.nsrc] = total;
-    total += n;
-    ++S.nsrc;
-  }
-  S.start[S.nsrc] = total;
+  // ---- every rank's gradient, addressable by the peers inside its rank's arena
+  NDArray src;
+  const RspSources S = RankSources(g, e.key, src_in, &src);
+  const int64_t total = S.start[S.nsrc];
   // optimizer state of the shard
   const bool need1 = U.opt == kOptSGD || U.opt == kOptAdam, need2 = U.opt == kOptAdam;
   DevState& st8 = e.rsp_shard_state[0];
-  for (int which = 0; which < 2; ++which) {
-    NDArray& a = which == 0 ? st8.s1 : st8.s2;
-    if (!(which == 0 ? need1 : need2) || !a.is_none()) continue;
-    a = NDArray(e.rsp_shards[0].shape(), Context::GPU(dev), kFloat32);
-    DeviceGuard gd(dev);
-    eng->BeginWrite(dev, *a.var());   // first writer of a possibly recycled block
-    KV_CUDA(cudaMemsetAsync(a.data(), 0, a.ByteSize(), eng->Stream(dev)));
-    eng->MarkWrite(dev, eng->Issue(dev), a.var());
+  if (need1 && st8.s1.is_none()) st8.s1 = ZerosOn(e.rsp_shards[0].shape(), dev, kFloat32);
+  if (need2 && st8.s2.is_none()) st8.s2 = ZerosOn(e.rsp_shards[0].shape(), dev, kFloat32);
+  const bool run = total > 0 && hi > lo;
+  NDArray d_nnr, ws;
+  if (run) {
+    d_nnr = NDArray({1}, Context::GPU(dev), kInt64);
+    ws = NDArray({static_cast<int64_t>(RspMergeWorkspaceBytes(total, BitsFor(rows), S.nsrc, lo, hi))}, Context::GPU(dev), kUint8);
   }
-  eng->BeginRead(dev, *src.var());
-  eng->BeginWrite(dev, *e.rsp_shards[0].var());
-  if (need1) eng->BeginWrite(dev, *st8.s1.var());
-  if (need2) eng->BeginWrite(dev, *st8.s2.var());
+  // every wait is declared before barrier 1: none lands between the two barriers
+  LaneOp op(dev);
+  op.Read(src).Write(e.rsp_shards[0]).Write(d_nnr).Write(ws);
+  if (need1) op.Write(st8.s1);
+  if (need2) op.Write(st8.s2);
   // barrier 1: every rank's gradient is complete (its barrier kernel is stream-ordered behind the
   // producer) before anybody reads it through IPC
   GroupBarrier();
-  NDArray d_nnr, ws;
-  if (total > 0 && hi > lo) {
-    DeviceGuard gd(dev);
-    d_nnr = NDArray({1}, Context::GPU(dev), kInt64);
-    ws = NDArray({static_cast<int64_t>(RspMergeWorkspaceBytes(total, BitsFor(rows), S.nsrc, lo, hi))}, Context::GPU(dev), kUint8);
+  if (run) {
     RspUpdateLaunch Uj = U;
     Uj.row_len = row_len;
     Uj.w = static_cast<float*>(e.rsp_shards[0].data()) - lo * row_len;
     Uj.s1 = need1 ? static_cast<float*>(st8.s1.data()) - lo * row_len : nullptr;
     Uj.s2 = need2 ? static_cast<float*>(st8.s2.data()) - lo * row_len : nullptr;
     LaunchRspMerge(S, BitsFor(rows), row_len, nullptr, nullptr, static_cast<int64_t*>(d_nnr.data()),
-                   ws.data(), ws.ByteSize(), eng->Stream(dev), &Uj, lo, hi);
+                   ws.data(), ws.ByteSize(), op.stream(), &Uj, lo, hi);
     eng->CountLaunch("rsp_merge(rank shard)", total * 24);
     eng->CountLaunch("rsp_sum+update(rank shard)", 0);
   }
   // barrier 2: every rank has finished reading the peers' gradients (they may now be reused) and
   // updating its shard (a pull that follows sees the new rows on every rank)
   GroupBarrier();
-  const uint64_t seq = eng->Issue(dev);
-  eng->MarkRead(dev, seq, src.var());
-  eng->MarkWrite(dev, seq, e.rsp_shards[0].var());
-  if (need1) eng->MarkWrite(dev, seq, st8.s1.var());
-  if (need2) eng->MarkWrite(dev, seq, st8.s2.var());
-  if (!d_nnr.is_none()) {
-    eng->MarkWrite(dev, seq, d_nnr.var());
-    eng->MarkWrite(dev, seq, ws.var());
-  }
+  op.Issue();
 }
 
 }  // namespace b200kv

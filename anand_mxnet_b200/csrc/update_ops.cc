@@ -210,9 +210,8 @@ void RspUpdateOp(const Spec& spec, const std::vector<NDArray>& in, std::vector<N
       << n << ": out must be the weight itself (kWriteInplace is expected for sparse " << spec.name
       << ")";
 
-  const int dev = w.dev();
   Engine* eng = Engine::Get();
-  DeviceGuard guard(dev);
+  LaneOp lop(w.dev());
   std::vector<const NDArray*> fill;
   for (size_t i = 2; i < in.size(); ++i) {
     if (in[i].stype() == kRowSparseStorage && in[i].nnr() == 0) {
@@ -222,10 +221,10 @@ void RspUpdateOp(const Spec& spec, const std::vector<NDArray>& in, std::vector<N
   }
   const bool update = g.storage_initialized();
   if (!update && fill.empty()) return;  // an all-zero gradient changes nothing
-  if (update) eng->BeginRead(dev, *g.var());
-  eng->BeginWrite(dev, *w.var());
-  for (size_t i = 2; i < in.size(); ++i) eng->BeginWrite(dev, *in[i].var());
-  cudaStream_t st = eng->Stream(dev);
+  if (update) lop.Read(g);
+  lop.Write(w);
+  for (size_t i = 2; i < in.size(); ++i) lop.Write(in[i]);
+  cudaStream_t st = lop.stream();
   for (const NDArray* a : fill) {
     KV_CUDA(cudaMemsetAsync(a->data(), 0, static_cast<size_t>(rows) * a->RowLength() * sizeof(float), st));
     LaunchFillRowIds(a->row_ids(), rows, st);
@@ -243,10 +242,7 @@ void RspUpdateOp(const Spec& spec, const std::vector<NDArray>& in, std::vector<N
     eng->CountLaunch(spec.launch_name,
                      static_cast<uint64_t>(L.nnr) * (spec.bytes_per_elem * L.row_len + 8));
   }
-  const uint64_t seq = eng->Issue(dev);
-  if (update) eng->MarkRead(dev, seq, g.var());
-  eng->MarkWrite(dev, seq, w.var());
-  for (size_t i = 2; i < in.size(); ++i) eng->MarkWrite(dev, seq, in[i].var());
+  lop.Issue();
 }
 
 }  // namespace
@@ -360,19 +356,14 @@ bool UpdateOp(const std::string& n, const std::vector<NDArray>& in, std::vector<
   L.n = w.Size();
   L.out_is_w = out_is_w;
 
-  Engine* eng = Engine::Get();
-  DeviceGuard guard(dev);
-  eng->BeginRead(dev, *g.var());
-  if (!out_is_w) eng->BeginRead(dev, *w.var());
-  eng->BeginWrite(dev, *out.var());
-  for (int i = 2; i < spec->nin; ++i) eng->BeginWrite(dev, *in[i].var());
-  LaunchUpdateOp(L, eng->Stream(dev));
-  eng->CountLaunch(spec->launch_name, static_cast<uint64_t>(spec->bytes_per_elem) * L.n);
-  const uint64_t seq = eng->Issue(dev);
-  eng->MarkRead(dev, seq, g.var());
-  if (!out_is_w) eng->MarkRead(dev, seq, w.var());
-  eng->MarkWrite(dev, seq, out.var());
-  for (int i = 2; i < spec->nin; ++i) eng->MarkWrite(dev, seq, in[i].var());
+  LaneOp lop(dev);
+  lop.Read(g);
+  if (!out_is_w) lop.Read(w);
+  lop.Write(out);
+  for (int i = 2; i < spec->nin; ++i) lop.Write(in[i]);
+  LaunchUpdateOp(L, lop.stream());
+  Engine::Get()->CountLaunch(spec->launch_name, static_cast<uint64_t>(spec->bytes_per_elem) * L.n);
+  lop.Issue();
   return true;
 }
 
