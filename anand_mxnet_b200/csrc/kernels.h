@@ -206,7 +206,7 @@ void LaunchMultiLars(int n, float* out, const float* lrs, const float* wsq, cons
 // nag_mom_update, mp_nag_mom_update, signsgd_update, signum_update, rmsprop_update,
 // rmspropalex_update, ftml_update, ftrl_update (optimizer_op-inl.h:1061-1222, 1953-2158, 2344-2431)
 enum UpdOp : int { kUpdNAG = 0, kUpdMPNAG, kUpdSignSGD, kUpdSignum, kUpdRMSProp, kUpdRMSPropAlex,
-                   kUpdFTML, kUpdFtrl, kUpdAdaGrad };
+                   kUpdFTML, kUpdFtrl, kUpdAdaGrad, kUpdGroupAdaGrad };
 struct UpdateLaunch {
   int op = kUpdNAG;
   int dtype = 0;                 // of w / g / out: kFloat32, or kFloat16 / kBfloat16 for kUpdMPNAG
@@ -230,6 +230,9 @@ void LaunchUpdateOp(const UpdateLaunch& L, cudaStream_t stream);
 // row_sparse forms of ftrl_update and _sparse_adagrad_update (rowsparse_kernels.cu;
 // FtrlDnsRspDnsKernel, AdagradDnsRspDnsKernel: optimizer_op-inl.h:2186-2219, 2507-2531): float32,
 // one warp per gradient row, the same Step<OP> as the dense kernel. Rows not in gidx stay untouched.
+// kUpdGroupAdaGrad (_contrib_group_adagrad_update, GroupAdagradDnsRspKernel: contrib/
+// optimizer_op-inl.h:96-139): s[0] is the history, one float per table row; each row's sum of
+// squares is folded strictly left to right, as the reference's CPU loop rounds it.
 void LaunchRspRowUpdateOp(const UpdateLaunch& L, cudaStream_t stream);
 // FillDnsZerosRspImpl's id half (init_op.h:474-487): ids[i] = i for i < rows
 void LaunchFillRowIds(int64_t* ids, int64_t rows, cudaStream_t stream);

@@ -16,7 +16,7 @@ namespace b200kv {
 
 void PlanChunks(uint64_t goff, size_t size, uint32_t key_slot, int ndev, int owner_fixed,
                 std::vector<std::vector<ChunkDesc>>* per_slot);  // kvstore.cc
-// NAG / Signum / RMSProp / FTML / Ftrl / sparse AdaGrad operators; false when `name` is not one of them
+// NAG / Signum / RMSProp / FTML / Ftrl / sparse AdaGrad / GroupAdaGrad operators; false when `name` is not one of them
 bool UpdateOp(const std::string& name, const std::vector<NDArray>& in, std::vector<NDArray>* outputs,
               const Params& p);  // update_ops.cc
 
@@ -39,7 +39,7 @@ const std::map<std::string, OpInfo>& Registry() {
           // single-tensor operators of the callback route (update_ops.cc)
           "nag_mom_update", "mp_nag_mom_update", "signsgd_update", "signum_update", "rmsprop_update",
           "rmspropalex_update", "ftml_update", "ftrl_update", "_sparse_ftrl_update",
-          "_sparse_adagrad_update"}) {
+          "_sparse_adagrad_update", "_contrib_group_adagrad_update"}) {
       r[n] = OpInfo{n};
     }
   }

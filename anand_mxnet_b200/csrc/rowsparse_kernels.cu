@@ -164,6 +164,154 @@ __global__ void __launch_bounds__(kWarpsPerBlock * 32) rsp_row_update_kernel(con
   }
 }
 
+// ---- _contrib_group_adagrad_update: GroupAdagradDnsRspKernel<cpu> (contrib/optimizer_op-inl.h:96-139)
+//   gr_j = clip(g_j * rescale);  ssq = ((0 + gr_0^2) + gr_1^2) + ... + gr_{L-1}^2   (left fold)
+//   h[r] = h[r] + ssq / (float)L;   w_j = w_j - (lr * gr_j) / sqrt(h[r] + eps)
+// One warp per gradient row. The row is cut into tiles of kGaTile elements; lane k holds the
+// contiguous run [16k, 16k+16) of a tile in registers, so the fold order is lane 0's run, then lane
+// 1's, ...: every lane squares its run in parallel, then the running sum walks the lanes in order,
+// each lane adding its 16 squares with one rounding per add and handing the sum on by __shfl_sync.
+// Elements past the row's end hold +0.0f: the running sum is never -0.0f (it starts at +0.0f and
+// adds squares), so adding +0.0f leaves it bitwise unchanged. The chain is ~32 x (16 adds + 1
+// shuffle) deep per tile; other warps' row traffic, and for one-tile rows this warp's own L2
+// prefetches issued before the fold, cover it.
+constexpr int kGaPer = 16;
+constexpr int kGaTile = 32 * kGaPer;
+
+// lane's run of one tile of a row (`row` at the tile's first element, `n` elements left in the
+// row), +0.0f past the end; vector form: n % 4 == 0 and `row` 16-B aligned
+template <bool VEC, bool STREAM>
+__device__ __forceinline__ void GaLoad(const float* row, int64_t n, int lane, float (&x)[kGaPer]) {
+  const int64_t o = static_cast<int64_t>(lane) * kGaPer;
+  if (VEC) {
+#pragma unroll
+    for (int v = 0; v < kGaPer / 4; ++v) {
+      float4 f = make_float4(0.f, 0.f, 0.f, 0.f);
+      if (o + 4 * v < n) {
+        const float4* p = reinterpret_cast<const float4*>(row + o) + v;
+        f = STREAM ? __ldcs(p) : *p;
+      }
+      x[4 * v] = f.x; x[4 * v + 1] = f.y; x[4 * v + 2] = f.z; x[4 * v + 3] = f.w;
+    }
+  } else {
+#pragma unroll
+    for (int j = 0; j < kGaPer; ++j) x[j] = o + j < n ? (STREAM ? __ldcs(row + o + j) : row[o + j]) : 0.f;
+  }
+}
+
+template <bool VEC>
+__device__ __forceinline__ void GaStore(float* row, int64_t n, int lane, const float (&x)[kGaPer]) {
+  const int64_t o = static_cast<int64_t>(lane) * kGaPer;
+  if (VEC) {
+#pragma unroll
+    for (int v = 0; v < kGaPer / 4; ++v) {
+      if (o + 4 * v < n) {
+        reinterpret_cast<float4*>(row + o)[v] = make_float4(x[4 * v], x[4 * v + 1], x[4 * v + 2], x[4 * v + 3]);
+      }
+    }
+  } else {
+#pragma unroll
+    for (int j = 0; j < kGaPer; ++j) {
+      if (o + j < n) row[o + j] = x[j];
+    }
+  }
+}
+
+// L2 prefetch of a run of n (<= kGaTile) floats: one 128-B line per lane
+__device__ __forceinline__ void GaPrefetchL2(const float* p, int64_t n, int lane) {
+  if (lane * 32 < n + 31) {
+    asm volatile("prefetch.global.L2 [%0];" ::"l"(p + (lane * 32 < n ? lane * 32 : n - 1)));
+  }
+}
+
+// the rescaled and clipped gradient (get_grad_rescaled, :110-118), in place; the padding past the
+// row's end stays +0.0f whatever rescale_grad is (0 * inf would be NaN)
+__device__ __forceinline__ void GaRescale(const UpdateLaunch& a, int64_t n, int lane, float (&x)[kGaPer]) {
+  const int64_t o = static_cast<int64_t>(lane) * kGaPer;
+#pragma unroll
+  for (int j = 0; j < kGaPer; ++j) {
+    if (o + j < n) {
+      x[j] = __fmul_rn(x[j], a.rescale);
+      if (a.clip >= 0.f) x[j] = clipf(x[j], a.clip);
+    }
+  }
+}
+
+// continues the left fold `s` over one tile of n (> 0) elements; returns it in every lane
+__device__ __forceinline__ float GaFold(float s, const float (&gr)[kGaPer], int64_t n) {
+  const int lanes = n >= kGaTile ? 32 : static_cast<int>((n + kGaPer - 1) / kGaPer);
+  for (int k = 0; k < lanes; ++k) {
+    float t = s;  // only lane k's t is kept
+#pragma unroll
+    for (int j = 0; j < kGaPer; ++j) t = __fadd_rn(t, __fmul_rn(gr[j], gr[j]));
+    s = __shfl_sync(0xffffffffu, t, k);
+  }
+  return s;
+}
+
+// w_j - (lr * gr_j) / den
+__device__ __forceinline__ void GaStep(const UpdateLaunch& a, float den, const float (&gr)[kGaPer],
+                                       float (&w)[kGaPer]) {
+#pragma unroll
+  for (int j = 0; j < kGaPer; ++j) w[j] = __fsub_rn(w[j], __fdiv_rn(__fmul_rn(a.lr, gr[j]), den));
+}
+
+// ONE_TILE (row_len <= kGaTile): the gradient row stays in registers between the fold and the
+// update. Before the fold, the warp asks L2 for this row's weight and the next row's gradient
+// (prefetches hold no registers), so the loads after the fold find them there. Longer rows read
+// the gradient twice, tile by tile: once for the fold, once for the update.
+template <bool VEC, bool ONE_TILE>
+__global__ void __launch_bounds__(kWarpsPerBlock * 32, ONE_TILE ? 4 : 3) rsp_group_adagrad_kernel(const UpdateLaunch a) {
+  const int lane = threadIdx.x & 31;
+  const int64_t nwarps = static_cast<int64_t>(gridDim.x) * kWarpsPerBlock;
+  const int64_t len = a.row_len;
+  const float flen = static_cast<float>(len);  // ssq / row_length: float / (float)index_t
+  const float* g = static_cast<const float*>(a.g);
+  float* w = static_cast<float*>(a.out);
+  float* h = a.s[0];
+  int64_t r = static_cast<int64_t>(blockIdx.x) * kWarpsPerBlock + (threadIdx.x >> 5);
+  if (ONE_TILE) {
+    for (; r < a.nnr; r += nwarps) {
+      const int64_t row = a.gidx[r];
+      float* wp = w + row * len;
+      GaPrefetchL2(wp, len, lane);
+      float gr[kGaPer], wv[kGaPer];
+      GaLoad<VEC, true>(g + r * len, len, lane, gr);
+      if (r + nwarps < a.nnr) GaPrefetchL2(g + (r + nwarps) * len, len, lane);
+      const float h0 = h[row];
+      GaRescale(a, len, lane, gr);
+      const float hn = __fadd_rn(h0, __fdiv_rn(GaFold(0.f, gr, len), flen));
+      GaLoad<VEC, false>(wp, len, lane, wv);
+      GaStep(a, __fsqrt_rn(__fadd_rn(hn, a.eps)), gr, wv);
+      GaStore<VEC>(wp, len, lane, wv);
+      if (lane == 0) h[row] = hn;
+    }
+  } else {
+    for (; r < a.nnr; r += nwarps) {
+      const int64_t row = a.gidx[r];
+      const float* gp = g + r * len;
+      float* wp = w + row * len;
+      float s = 0.f, x[kGaPer];
+      for (int64_t b = 0; b < len; b += kGaTile) {
+        GaLoad<VEC, true>(gp + b, len - b, lane, x);
+        GaRescale(a, len - b, lane, x);
+        s = GaFold(s, x, len - b);
+      }
+      const float hn = __fadd_rn(h[row], __fdiv_rn(s, flen));
+      const float den = __fsqrt_rn(__fadd_rn(hn, a.eps));
+      for (int64_t b = 0; b < len; b += kGaTile) {
+        float wv[kGaPer];
+        GaLoad<VEC, true>(gp + b, len - b, lane, x);
+        GaLoad<VEC, false>(wp + b, len - b, lane, wv);
+        GaRescale(a, len - b, lane, x);
+        GaStep(a, den, x, wv);
+        GaStore<VEC>(wp + b, len - b, lane, wv);
+      }
+      if (lane == 0) h[row] = hn;
+    }
+  }
+}
+
 __global__ void fill_row_ids_kernel(int64_t* ids, int64_t rows) {
   const int64_t stride = static_cast<int64_t>(gridDim.x) * blockDim.x;
   for (int64_t i = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x; i < rows; i += stride) {
@@ -903,9 +1051,21 @@ void LaunchRspRowUpdateOp(const UpdateLaunch& L, cudaStream_t stream) {
   KV_CHECK(L.out == L.w) << "row_sparse optimizer operators update the weight in place";
   auto aligned = [](const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; };
   bool vec = L.row_len % 4 == 0 && aligned(L.g) && aligned(L.out);
-  for (int k = 0; k < NumStates(L.op); ++k) vec = vec && aligned(L.s[k]);
   const int blocks = static_cast<int>(std::min<int64_t>((L.nnr + kWarpsPerBlock - 1) / kWarpsPerBlock,
                                                         kNumSMs * 16));
+  if (L.op == kUpdGroupAdaGrad) {  // one history value per row: only g and w move along the row
+    const dim3 grid(blocks), block(kWarpsPerBlock * 32);
+    if (L.row_len <= kGaTile) {
+      if (vec) rsp_group_adagrad_kernel<true, true><<<grid, block, 0, stream>>>(L);
+      else rsp_group_adagrad_kernel<false, true><<<grid, block, 0, stream>>>(L);
+    } else {
+      if (vec) rsp_group_adagrad_kernel<true, false><<<grid, block, 0, stream>>>(L);
+      else rsp_group_adagrad_kernel<false, false><<<grid, block, 0, stream>>>(L);
+    }
+    KV_CUDA(cudaGetLastError());
+    return;
+  }
+  for (int k = 0; k < NumStates(L.op); ++k) vec = vec && aligned(L.s[k]);
   switch (L.op) {
     case kUpdFtrl: rsp_row_update_kernel<kUpdFtrl><<<blocks, kWarpsPerBlock * 32, 0, stream>>>(L, vec); break;
     case kUpdAdaGrad: rsp_row_update_kernel<kUpdAdaGrad><<<blocks, kWarpsPerBlock * 32, 0, stream>>>(L, vec); break;

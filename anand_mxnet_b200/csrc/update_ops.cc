@@ -1,8 +1,8 @@
 // update_ops.cc -- host side of the single-tensor optimizer operators that the reference's NAG,
 // Signum, RMSProp, FTML and Ftrl optimizers call from their `update` (the per-key updater callback
 // of the store, and the local updaters of update_on_kvstore=False), plus the row_sparse forms of
-// ftrl_update and AdaGrad's _sparse_adagrad_update. Kernels: update_kernels.cu (dense),
-// rowsparse_kernels.cu (row_sparse).
+// ftrl_update, AdaGrad's _sparse_adagrad_update and GroupAdaGrad's _contrib_group_adagrad_update.
+// Kernels: update_kernels.cu (dense), rowsparse_kernels.cu (row_sparse).
 //
 // Reference operator definitions (inputs, parameter structs, kernels):
 //   nag_mom_update, mp_nag_mom_update    src/operator/optimizer_op.cc:712-762, optimizer_op-inl.h:1032-1160
@@ -11,6 +11,7 @@
 //   ftrl_update, _sparse_ftrl_update     optimizer_op.cc:854-893, optimizer_op-inl.h:2101-2314
 //   signsgd_update, signum_update        optimizer_op.cc:49-104, optimizer_op-inl.h:2319-2452
 //   _sparse_adagrad_update               optimizer_op.cc:895-924, optimizer_op-inl.h:2454-2649
+//   _contrib_group_adagrad_update        contrib/optimizer_op.cc:53-86, contrib/optimizer_op-inl.h:46-243
 //
 // Dense float32 arrays (mp_nag_mom_update: float16 / bfloat16 weights with float32 mom and
 // weight32), or the row_sparse forms in float32 (RspUpdateOp). The reference would densify a
@@ -49,6 +50,8 @@ const Spec kSpecs[] = {
     // and AdaGrad's operator (optimizer_op.cc:895-924, optimizer_op-inl.h:2454-2649)
     {"_sparse_ftrl_update", kUpdFtrl, 4, "update_op(ftrl_update)", 28},
     {"_sparse_adagrad_update", kUpdAdaGrad, 3, "update_op(_sparse_adagrad_update)", 20},
+    // GroupAdaGrad's operator: g 4 + w 4+4 per element; the history is one float per row
+    {"_contrib_group_adagrad_update", kUpdGroupAdaGrad, 3, "update_op(_contrib_group_adagrad_update)", 12},
 };
 
 // Restatement of dmlc::stod == ParseFloat<double, true> (3rdparty/dmlc-core/include/dmlc/
@@ -148,13 +151,15 @@ float InRange(float v, const char* key, float lo, float hi) {
 
 const char* StypeName(int stype) { return stype == kRowSparseStorage ? "row_sparse" : "default"; }
 
-// ftrl_update (FtrlUpdateEx, optimizer_op-inl.h:2291-2314) and _sparse_adagrad_update
-// (AdagradStorageType / AdagradUpdateEx, 2480-2501, 2620-2649) with row_sparse operands: only the
-// rows listed in the gradient move. Every check runs before anything is enqueued, so a refused
-// call leaves all operands as they were. Accepted forms:
+// ftrl_update (FtrlUpdateEx, optimizer_op-inl.h:2291-2314), _sparse_adagrad_update
+// (AdagradStorageType / AdagradUpdateEx, 2480-2501, 2620-2649) and _contrib_group_adagrad_update
+// (GroupAdagradStorageType / GroupAdagradUpdateEx, contrib/optimizer_op-inl.h:67-93, 216-242) with
+// row_sparse operands: only the rows listed in the gradient move. Every check runs before anything
+// is enqueued, so a refused call leaves all operands as they were. Accepted forms:
 //   ftrl_update / _sparse_ftrl_update   (row_sparse weight, grad, z, n)
 //   _sparse_adagrad_update              (row_sparse weight, grad, history), wd == 0
 //                                       (dense weight, row_sparse grad, dense history), wd == 0
+//   _contrib_group_adagrad_update       the same two forms; history has one value per row
 void RspUpdateOp(const Spec& spec, const std::vector<NDArray>& in, std::vector<NDArray>* outputs,
                  const Params& p) {
   const std::string n = spec.name;
@@ -175,6 +180,21 @@ void RspUpdateOp(const Spec& spec, const std::vector<NDArray>& in, std::vector<N
     KV_CHECK(wst == kRowSparseStorage && g.stype() == kRowSparseStorage)
         << n << ": the row_sparse form needs row_sparse weight, grad, z and n (a dense weight with a "
         << "row_sparse gradient is not supported)";
+  } else if (op == kUpdGroupAdaGrad) {  // GroupAdagradParam (contrib/optimizer_op-inl.h:46-65)
+    for (const auto& kv : p) {  // dmlc::Parameter::Init rejects unknown keys (wd among them)
+      KV_CHECK(kv.first == "lr" || kv.first == "rescale_grad" || kv.first == "clip_gradient" ||
+               kv.first == "epsilon")
+          << "Cannot find argument '" << kv.first << "', Possible Arguments: lr, rescale_grad, "
+          << "clip_gradient, epsilon";
+    }
+    L.eps = GetF(p, "epsilon", 1.0e-5f);
+    const int hst = in[2].stype();
+    // all-dense operands dispatch to an FCompute the reference does not register
+    KV_CHECK(g.stype() == kRowSparseStorage || wst != kDefaultStorage || hst != kDefaultStorage)
+        << "Operator " << n << " is not implemented for GPU (dense weight, grad and history)";
+    KV_CHECK(g.stype() == kRowSparseStorage && hst == wst)  // GroupAdagradStorageType (:67-93)
+        << "Operator not implemented: operator = " << n << "\ninput storage types = ["
+        << StypeName(wst) << ", " << StypeName(g.stype()) << ", " << StypeName(hst) << ", ]";
   } else {  // AdagradParam; AdagradUpdateDnsRspDnsImpl (2569-2570) checks wd first
     L.eps = GetF(p, "epsilon", 1.0e-7f);
     KV_CHECK(L.wd == 0.f) << "sparse adagrad_update does not support wd.";
@@ -183,16 +203,24 @@ void RspUpdateOp(const Spec& spec, const std::vector<NDArray>& in, std::vector<N
         << "row_sparse, default), got (" << StypeName(wst) << ", " << StypeName(g.stype()) << ", "
         << StypeName(in[2].stype()) << ")";
   }
-  for (const NDArray& a : in) {
+  KV_CHECK(!w.shape().empty()) << n << ": the weight needs at least one dimension";
+  const int64_t rows = w.shape()[0];
+  for (size_t i = 0; i < in.size(); ++i) {
+    const NDArray& a = in[i];
     KV_CHECK(a.on_gpu() && a.dev() == w.dev()) << n << ": all operands must be on the same GPU";
     KV_CHECK_EQ(a.dtype(), kFloat32) << n << ": row_sparse updates run on float32 arrays only, got "
                                      << DTypeName(a.dtype());
-    KV_CHECK(a.shape() == w.shape()) << n << ": weight / grad / state shape mismatch";
+    if (op == kUpdGroupAdaGrad && i == 2) {
+      // GroupAdagradShape (contrib/optimizer_op.cc:37-51) checks only history.shape[0]; the kernel
+      // addresses one value per row, so a wider history is refused here
+      KV_CHECK(!a.shape().empty() && a.shape()[0] == rows && a.Size() == static_cast<size_t>(rows))
+          << n << ": history must hold one value per weight row, e.g. shape (" << rows << ", 1)";
+    } else {
+      KV_CHECK(a.shape() == w.shape()) << n << ": weight / grad / state shape mismatch";
+    }
   }
-  KV_CHECK(!w.shape().empty()) << n << ": the weight needs at least one dimension";
-  const int64_t rows = w.shape()[0];
   // CheckAllRowsPresent (operator_common.h:500-511)
-  const char* func = op == kUpdFtrl ? "FtrlUpdate" : "AdagradUpdate";
+  const char* func = op == kUpdFtrl ? "FtrlUpdate" : op == kUpdAdaGrad ? "AdagradUpdate" : "GroupAdagradUpdate";
   KV_CHECK(wst != kRowSparseStorage || w.nnr() == rows)
       << func << " for RowSparse weights is only implemented for RowSparse weights with all rows "
       << "containing non-zeros. Expects weights.data.shape[0] (" << w.nnr() << ") == weights.shape[0] ("
@@ -239,8 +267,10 @@ void RspUpdateOp(const Spec& spec, const std::vector<NDArray>& in, std::vector<N
     L.row_len = static_cast<int64_t>(w.RowLength());
     for (size_t i = 2; i < in.size(); ++i) L.s[i - 2] = static_cast<float*>(in[i].data());
     LaunchRspRowUpdateOp(L, st);
+    // + 8 B of id per row, and GroupAdaGrad's history value read and written
+    const int64_t per_row = op == kUpdGroupAdaGrad ? 16 : 8;
     eng->CountLaunch(spec.launch_name,
-                     static_cast<uint64_t>(L.nnr) * (spec.bytes_per_elem * L.row_len + 8));
+                     static_cast<uint64_t>(L.nnr) * (spec.bytes_per_elem * L.row_len + per_row));
   }
   lop.Issue();
 }
@@ -265,7 +295,7 @@ bool UpdateOp(const std::string& n, const std::vector<NDArray>& in, std::vector<
           << in[i].stype() << " and weight.stype = " << w.stype();
     }
   }
-  if (op == kUpdAdaGrad || w.stype() == kRowSparseStorage) {
+  if (op == kUpdAdaGrad || op == kUpdGroupAdaGrad || w.stype() == kRowSparseStorage) {
     RspUpdateOp(*spec, in, outputs, p);
     return true;
   }

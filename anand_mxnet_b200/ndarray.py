@@ -652,5 +652,9 @@ class _Contrib(object):
                                                step_count=step_count, learning_rates=lrs, wds=wds,
                                                **kwargs)
 
+    # GroupAdaGrad's lazy row update (float32, out must be the weight): (row_sparse, row_sparse,
+    # row_sparse) or (dense, row_sparse, dense), history of shape (rows, 1); no wd parameter
+    group_adagrad_update = staticmethod(_op('_contrib_group_adagrad_update'))
+
 
 contrib = _Contrib()

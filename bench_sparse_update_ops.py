@@ -1,6 +1,7 @@
 #!/usr/bin/env python
 """bench_sparse_update_ops.py -- the row_sparse forms of ftrl_update and _sparse_adagrad_update
-(rowsparse_kernels.cu: rsp_row_update_kernel) on one GPU, on an embedding table of --rows x --row-len
+(rowsparse_kernels.cu: rsp_row_update_kernel) and GroupAdaGrad's _contrib_group_adagrad_update
+(rsp_group_adagrad_kernel) on one GPU, on an embedding table of --rows x --row-len
 float32 (default 1 M x 512) with --nnr (default 80 000) seeded unique gradient rows.
 
 Workloads, each timed with CUDA events over --iters launches after --warmup:
@@ -10,14 +11,19 @@ Workloads, each timed with CUDA events over --iters launches after --warmup:
   store_ftrl_step    one step of a row_sparse key through the store's callback route with the
                      tests/compat Ftrl: a push of 8 values of nnr/8 rows each (disjoint row sets),
                      the merge, the updater's ftrl_update, and a row_sparse_pull of the nnr rows
+  group_adagrad_rsp  _contrib_group_adagrad_update, (row_sparse, row_sparse, row_sparse), history
+                     (rows, 1)
+  group_adagrad_dns  _contrib_group_adagrad_update, (dense, row_sparse, dense)
+  store_group_adagrad_step  store_ftrl_step with the tests/compat GroupAdaGrad
 
 Before timing, the first call of every workload is checked bit for bit against the numpy
 restatement of the reference kernel (oracle/golden_sparse_update_ops.py, which tests hold to the
 reference's own code) on the touched rows, and a sample of untouched rows is checked unchanged; the
 run fails if any differs. One JSON line per workload: time, algorithmic GB/s of the update (bytes per
-touched element: Ftrl 28 = g 4 + w 4+4 + z 8 + n 8; AdaGrad 20 = g 4 + w 8 + h 8; plus 8 bytes of id
-per row) and its fraction of the 3.35 TB/s H100 SXM data-sheet bandwidth (a bound that was not
-measured), with the card's name and power limit.
+touched element: Ftrl 28 = g 4 + w 4+4 + z 8 + n 8; AdaGrad 20 = g 4 + w 8 + h 8; GroupAdaGrad 12 =
+g 4 + w 8; plus per row 8 bytes of id, and for GroupAdaGrad 8 more for its history value) and its
+fraction of the 3.35 TB/s H100 SXM data-sheet bandwidth (a bound that was not measured), with the
+card's name and power limit.
 """
 import argparse
 import ctypes
@@ -34,9 +40,11 @@ sys.path.insert(0, os.path.join(ROOT, "oracle"))
 sys.path.insert(0, os.path.join(ROOT, "tests"))
 
 HBM_DATASHEET_GBS = 3350.0
-BYTES = {'ftrl': 28, 'adagrad': 20}
+BYTES = {'ftrl': 28, 'adagrad': 20, 'group_adagrad': 12}
+ROW_BYTES = {'ftrl': 8, 'adagrad': 8, 'group_adagrad': 16}
 FTRL = dict(lr=0.1, lamda1=0.01, beta=1.0, wd=0.0, rescale_grad=1.0)
 ADAGRAD = dict(lr=0.05, epsilon=1e-07, wd=0.0, rescale_grad=1.0)
+GROUP_ADAGRAD = dict(lr=0.05, epsilon=1e-05, rescale_grad=1.0)
 
 
 def card():
@@ -58,6 +66,7 @@ def main():
     import anand_mxnet_b200 as mx
     from anand_mxnet_b200.base import _LIB, check_call
     import golden_sparse_update_ops as GS
+    import golden_group_adagrad as GG
     name, plim = card()
     stream = torch.cuda.Stream()
     torch.cuda.set_stream(stream)
@@ -118,7 +127,7 @@ def main():
             failed.append(workload)
 
     def emit(workload, kind, ms, extra=None):
-        nbytes = N * (BYTES[kind] * L + 8)
+        nbytes = N * (BYTES[kind] * L + ROW_BYTES[kind])
         gbs = nbytes / (ms * 1e-3) / 1e9
         print(json.dumps({"metric": "sparse_update_GBps", "workload": workload, "value": gbs, "unit": "GB/s",
                           "ms": ms, "table": [R, L], "rows_updated": N, "bytes": nbytes,
@@ -186,6 +195,71 @@ def main():
     emit("store_ftrl_step", 'ftrl', timed(store_step),
          {"note": "whole step: push of 8 values + merge + callback ftrl_update + row_sparse_pull; "
                   "GB/s counts the update's bytes only"})
+    del kv, vals, out, st
+    torch.cuda.empty_cache()
+
+    # ------------------------------------------------------------------------------ GroupAdaGrad
+    def hist(t, stype):
+        """a (rows, 1) history: row_sparse holding every row, or dense"""
+        if stype == 'default':
+            return mx.nd.from_torch(t)
+        out = mx.nd.sparse.zeros('row_sparse', (R, 1), mx.gpu(0))
+        d, i = mx.nd.from_torch(t), mx.nd.from_torch(torch.arange(R, device='cuda'))
+        check_call(_LIB.MXNDArraySyncCopyFromNDArray(out.handle, d.handle, ctypes.c_int(-1)))
+        check_call(_LIB.MXNDArraySyncCopyFromNDArray(out.handle, i.handle, ctypes.c_int(0)))
+        return out
+
+    def hvals(a):
+        return mx.nd.to_torch(a.data if a.stype == 'row_sparse' else a).view(R, 1)
+
+    def group_parity(workload, w_before, h_before, w, h, h_cold):
+        """the restatement on the touched rows; sampled cold rows of w and h unchanged"""
+        tw, th = w_before.index_select(0, ids).cpu().numpy(), h_before.index_select(0, ids).cpu().numpy()
+        GG.restate(GG.OP, [1, 1, 1], [N, N, N], [tw, gvals.cpu().numpy(), th], np.arange(N), N, L, True,
+                   **GROUP_ADAGRAD)
+        ok = all(np.array_equal(a.index_select(0, ids).cpu().numpy().view(np.uint32), t.view(np.uint32))
+                 for a, t in ((w, tw), (h, th)))
+        ok = ok and torch.equal(w.index_select(0, cold).view(torch.int32),
+                                w_before.index_select(0, cold).view(torch.int32))
+        ok = ok and torch.equal(h.index_select(0, cold).view(torch.int32), h_cold.view(torch.int32))
+        print(json.dumps({"parity": workload, "bit_exact": bool(ok)}))
+        if not ok:
+            failed.append(workload)
+
+    f = mx.nd.contrib.group_adagrad_update
+    for workload, stype in [('group_adagrad_rsp', 'row_sparse'), ('group_adagrad_dns', 'default')]:
+        w0, h0 = uniform(-1, 1, R, L), uniform(0, 1, R, 1)
+        w, h = table(w0, stype), hist(h0, stype)
+        w_before, h_before = tensor(w).clone(), hvals(h).clone()
+        del w0, h0
+        f(w, g, h, out=w, **GROUP_ADAGRAD)
+        mx.nd.waitall()
+        group_parity(workload, w_before, h_before, tensor(w), hvals(h), h_before.index_select(0, cold))
+        del w_before, h_before
+        emit(workload, 'group_adagrad', timed(lambda: f(w, g, h, out=w, **GROUP_ADAGRAD)))
+        del w, h
+        torch.cuda.empty_cache()
+
+    from compat import mxnet_optimizer_contrib as mxopt_contrib
+    w0 = uniform(-1, 1, R, L)
+    kv = mx.kv.create('device')
+    kv.init(0, table(w0, 'row_sparse'))
+    kv.set_optimizer(mxopt_contrib.GroupAdaGrad(learning_rate=GROUP_ADAGRAD['lr'],
+                                                eps=GROUP_ADAGRAD['epsilon']))
+    vals = [rsp(gvals.index_select(0, torch.from_numpy(np.sort(p)).cuda()),
+                ids.index_select(0, torch.from_numpy(np.sort(p)).cuda())) for p in parts]
+    out = mx.nd.sparse.zeros('row_sparse', shape, mx.gpu(0))
+    store_step()
+    mx.nd.waitall()
+    # the pulled rows and the history's touched rows against the restatement; cold history rows 0
+    w_after = w0.clone()
+    w_after.index_copy_(0, ids, mx.nd.to_torch(out.data).view(N, L))
+    group_parity("store_group_adagrad_step", w0, torch.zeros(R, 1, device='cuda'), w_after,
+                 hvals(kv._updater.states[0]), torch.zeros(len(cold), 1, device='cuda'))
+    del w_after
+    emit("store_group_adagrad_step", 'group_adagrad', timed(store_step),
+         {"note": "whole step: push of 8 values + merge + callback group_adagrad_update + "
+                  "row_sparse_pull; GB/s counts the update's bytes only"})
     if failed:
         print(json.dumps({"parity_failed": failed}))
         sys.exit(1)
