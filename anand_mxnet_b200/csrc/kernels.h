@@ -165,6 +165,21 @@ void LaunchUniqueBatch(const RetainItem* h_items, int nitems, int64_t total_ids,
 void LaunchRetainBatch(int nitems, int64_t total_ids, int id_bits, const int64_t* d_off,
                        void* workspace, cudaStream_t stream);
 
+// whole-value pull of a row_sparse value (CopyFromTo with storage casts, ndarray.cc:1076-1093,
+// cast_storage-inl.h:74-140), every target in one pass: row_sparse targets get the nnr ids and
+// rows, dense targets every table row (the stored row or zeros). Rows move in 16-byte units when
+// row_bytes and every base are 16-byte aligned, else in 4- or 1-byte units; any dtype.
+struct RspBroadcastLaunch {
+  const int64_t* src_idx = nullptr;  // nnr ascending ids
+  const void* src_val = nullptr;     // nnr rows of row_bytes
+  int64_t nnr = 0, rows = 0, row_bytes = 0;
+  int n_rsp = 0, n_dns = 0;
+  int64_t* rsp_idx[kMaxDst] = {};    // row_sparse targets with room for nnr rows
+  void* rsp_val[kMaxDst] = {};
+  void* dns[kMaxDst] = {};           // dense targets of rows x row_bytes
+};
+void LaunchRspBroadcast(const RspBroadcastLaunch& p, cudaStream_t stream);
+
 // ---- multi-tensor optimizer operators (multi_tensor_kernels.cu; SURVEY 8f-f1) ----
 constexpr int kMTChunk = 8192;      // elements per CTA
 constexpr int kMTMaxTensors = 64;   // tensors per launch (their scalars travel by value)

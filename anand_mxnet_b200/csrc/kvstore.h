@@ -53,7 +53,10 @@ struct KeyEntry {
   int key = 0;
   std::vector<int64_t> shape;
   int dtype = kFloat32;
-  int stype = kDefaultStorage;
+  int stype = kDefaultStorage;   // as initialised
+  // storage type of the current value: a dense key holds a row_sparse value (in `rsp`) after a
+  // row_sparse push without an updater (kvstore_local.h:237-243), until its next dense push
+  int vstype = kDefaultStorage;
   size_t size = 0;
   uint64_t goff = 0;    // offset in the store-global element space
   NDArray host;         // value as initialised, pinned host (kvstore_local.h:202) until first GPU use
@@ -62,7 +65,7 @@ struct KeyEntry {
   std::map<int, DevState> dev;
   uint8_t queued = 0;   // deferred bucket execution: bit 0 = a push of this key is queued, bit 1 = a pull
   NDArray merged;       // reduce target of the updater-callback path (on `home`)
-  NDArray rsp;          // row_sparse stored value (on `home` or host)
+  NDArray rsp;          // row_sparse stored value (on `home` or host), see vstype
   // Row-range sharding of a row_sparse table whose stored value holds every row and whose
   // optimizer runs fused on the store (the embedding-training case, SURVEY 8e): GPU rsp_devs[j]
   // owns rows [j*rsp_rows_per, (j+1)*rsp_rows_per) of the weight and of the optimizer state.
@@ -222,6 +225,8 @@ class KVStore {
   bool RunCachedCall(const std::vector<uint64_t>& sig);
   void StoreCachedCall(const std::vector<uint64_t>& sig, std::vector<Prepared>&& launches);
   void ExecCallbackPush(KeyEntry& e, const std::vector<NDArray>& srcs);
+  void DensifyValue(KeyEntry& e);                       // dense key: row_sparse value -> dense weight
+  NDArray RowSparseValue(KeyEntry& e, const std::vector<NDArray>& outs);  // whole, on a GPU
   void EnsureOnDevice(KeyEntry& e, int dev);            // HOST -> WHOLE(dev)
   void EnsureStriped(KeyEntry& e);                      // WHOLE -> STRIPED(devset_)
   void EnsureWhole(KeyEntry& e, int dev);               // STRIPED -> WHOLE(dev)
@@ -259,6 +264,7 @@ class KVStore {
   bool dist_ = false;         // created inside a one-rank-per-GPU peer group
   int stage_gen_ = 0;         // staging-buffer generation of the call being prepared / replayed (0 / 1)
   bool nccl_ = false;         // cross-rank sums go through ncclAllReduce (type 'nccl', or no peer memory)
+  bool nccl_type_ = false;    // created as 'nccl': dense values only (src/kvstore/kvstore_nccl.h:62-70)
   int rank_ = 0, group_size_ = 1;
   bool order_local_ = true;   // 'local' => CommCPU association, 'device' => left fold
   int key_type_ = -1;         // -1 undefined, 0 string, 1 int (kvstore_local.h:60-64)

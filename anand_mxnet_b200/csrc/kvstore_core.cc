@@ -10,6 +10,7 @@
 
 #include "group.h"
 #include "nccl_dyn.h"
+#include "rowsparse.h"
 #include "scalar_parse.h"
 
 namespace b200kv {
@@ -68,6 +69,7 @@ KVStore::KVStore(const std::string& type) : type_(type) {
       << "kvstore type '" << type << "': multi-node parameter-server stores are outside this "
       << "library (single-node 'local' / 'device' / 'nccl' only)";
   order_local_ = !(t.find("device") != std::string::npos || t.find("nccl") != std::string::npos);
+  nccl_type_ = t.find("nccl") != std::string::npos;
   Engine::Get()->NumDevices();  // fails loudly when there is no GPU
   if (PeerGroup* g = PeerGroup::Get()) {
     // one rank per GPU: this store is one worker of a group (the role dist_device_sync plays in
@@ -164,6 +166,7 @@ void KVStore::InitImpl(const std::vector<int>& keys, const std::vector<NDArray>&
     e->shape = v.shape();
     e->dtype = v.dtype();
     e->stype = v.stype();
+    e->vstype = v.stype();
     e->size = v.Size();
     e->goff = next_goff_;
     next_goff_ += RoundUp(std::max<size_t>(e->size, 1), kKeyAlignElems);
@@ -395,7 +398,7 @@ bool KVStore::TryDefer(int kind, std::vector<int>& vkeys, std::vector<NDArray>& 
     KeyEntry& e = (last != nullptr && last->key == vkeys[i]) ? *last : Entry(vkeys[i]);  // un-initialised keys still fail synchronously
     last = &e;
     const NDArray& v = values[i];
-    if (v.stype() != kDefaultStorage || e.stype != kDefaultStorage) return false;
+    if (v.stype() != kDefaultStorage || e.vstype != kDefaultStorage) return false;
     KV_CHECK_EQ(v.Size(), e.size) << "push: shape mismatch for key " << e.key;
     KV_CHECK_EQ(v.dtype(), e.dtype) << "push: dtype mismatch for key " << e.key;
     bytes += v.ByteSize();
@@ -405,7 +408,7 @@ bool KVStore::TryDefer(int kind, std::vector<int>& vkeys, std::vector<NDArray>& 
     KeyEntry& e = (last != nullptr && last->key == okeys[i]) ? *last : Entry(okeys[i]);
     last = &e;
     const NDArray& o = outs[i];
-    if (o.stype() != kDefaultStorage || e.stype != kDefaultStorage) return false;
+    if (o.stype() != kDefaultStorage || e.vstype != kDefaultStorage) return false;
     KV_CHECK_EQ(o.Size(), e.size) << "pull: shape mismatch for key " << e.key;
     KV_CHECK_EQ(o.dtype(), e.dtype) << "pull: dtype mismatch for key " << e.key;
     bytes += o.ByteSize();
@@ -576,6 +579,18 @@ void KVStore::PushImpl(const std::vector<int>& keys, const std::vector<NDArray>&
     if (srcs[0].stype() == kRowSparseStorage) {
       for (auto& s : srcs) KV_CHECK_EQ(s.stype(), kRowSparseStorage) << "mixed storage types in push";
       PushRowSparse(e, srcs);   // one rank per GPU: PushRowSparseGroup (row-range shards per rank)
+      // a dense key's pull side: the value left by the push, dense or row_sparse
+      auto oit = out_of.find(e.key);
+      if (e.stype == kDefaultStorage && oit != out_of.end()) {
+        if (e.vstype == kRowSparseStorage) {
+          BroadcastRspValue(RowSparseValue(e, ogrouped[oit->second]), ogrouped[oit->second]);
+        } else {
+          DenseOp p;
+          p.e = &e;
+          p.outs = ogrouped[oit->second];
+          pulls.push_back(p);
+        }
+      }
       continue;
     }
     KV_CHECK_EQ(e.stype, kDefaultStorage)
@@ -589,6 +604,7 @@ void KVStore::PushImpl(const std::vector<int>& keys, const std::vector<NDArray>&
     auto oit = out_of.find(e.key);
     KV_CHECK(!(callback && dist_))
         << "the one-rank-per-GPU store runs fused optimizers only (sgd / adam / test) or no updater";
+    DensifyValue(e);
     if (callback) {
       ExecCallbackPush(e, srcs);
       if (oit != out_of.end()) {
@@ -609,6 +625,10 @@ void KVStore::PushImpl(const std::vector<int>& keys, const std::vector<NDArray>&
   for (size_t i = 0; i < ouniq.size(); ++i) {
     if (pushed.count(ouniq[i])) continue;
     KeyEntry& e = Entry(ouniq[i]);
+    if (e.vstype == kRowSparseStorage) {
+      BroadcastRspValue(RowSparseValue(e, ogrouped[i]), ogrouped[i]);
+      continue;
+    }
     DenseOp p;
     p.e = &e;
     p.outs = ogrouped[i];
@@ -641,23 +661,19 @@ void KVStore::PullImpl(const std::vector<int>& keys, const std::vector<NDArray>&
   std::vector<DenseOp> pulls;
   for (size_t i = 0; i < uniq.size(); ++i) {
     KeyEntry& e = Entry(uniq[i]);
-    bool plain = e.stype == kDefaultStorage;
+    bool plain = e.vstype == kDefaultStorage;
     for (auto& o : grouped[i]) plain = plain && o.stype() == kDefaultStorage;
     if (!plain) {
       // a row_sparse key or a row_sparse target: Comm::Broadcast degenerates to CopyFromTo with a
       // storage cast (comm.h:598-616, ndarray.cc:1147-1196) -- the whole stored value travels
       cacheable_call = false;
-      NDArray local;
-      if (e.stype == kRowSparseStorage) {
-        KV_CHECK(!e.rsp_group) << "key " << e.key << ": a whole-value pull of a row_sparse table that is "
-                               << "sharded over the ranks is not supported; use row_sparse_pull";
-        UnshardRsp(e);
-        local = e.rsp;
-      } else {
-        const int dev = e.striped ? devset_[0] : (e.home >= 0 ? e.home : (devset_.empty() ? 0 : devset_[0]));
-        EnsureWhole(e, dev);
-        local = e.dev[e.home].w;
+      if (e.vstype == kRowSparseStorage) {
+        BroadcastRspValue(RowSparseValue(e, grouped[i]), grouped[i]);
+        continue;
       }
+      const int dev = e.striped ? devset_[0] : (e.home >= 0 ? e.home : (devset_.empty() ? 0 : devset_[0]));
+      EnsureWhole(e, dev);
+      const NDArray local = e.dev[e.home].w;
       for (auto& o : grouped[i]) CopyFromTo(local, o);
       continue;
     }
@@ -980,6 +996,30 @@ void KVStore::ExecCallbackPush(KeyEntry& e, const std::vector<NDArray>& srcs_in)
   } else {
     updater_(e.key, recv_h, local_h, updater_handle_);
   }
+}
+
+// A dense key whose value is row_sparse (a row_sparse push without an updater) takes it back into
+// its dense weight -- zeros plus the stored rows -- before anything reads or updates that weight.
+void KVStore::DensifyValue(KeyEntry& e) {
+  if (e.vstype == kDefaultStorage) return;
+  BroadcastRspValue(e.rsp, {e.dev[e.home].w});
+  e.rsp = NDArray();
+  e.vstype = kDefaultStorage;
+  ++layout_epoch_;
+}
+
+// The row_sparse value of a key on a GPU, whole: a table sharded over this process's GPUs is folded
+// back onto its home; a value still on the host is copied to the GPU of the first GPU out.
+NDArray KVStore::RowSparseValue(KeyEntry& e, const std::vector<NDArray>& outs) {
+  KV_CHECK(!e.rsp_group) << "key " << e.key << ": a whole-value pull of a row_sparse table that is "
+                         << "sharded over the ranks is not supported; use row_sparse_pull";
+  UnshardRsp(e);
+  if (e.rsp.on_gpu()) return e.rsp;
+  int dev = 0;
+  for (auto& o : outs) {
+    if (o.on_gpu()) { dev = o.dev(); break; }
+  }
+  return e.rsp.Copy(Context::GPU(dev));
 }
 
 // =================================================================================================

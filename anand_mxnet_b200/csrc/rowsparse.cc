@@ -106,27 +106,47 @@ RspSources RankSources(PeerGroup* g, int64_t key, const NDArray& src_in, NDArray
 
 }  // namespace
 
+// A dense key takes row_sparse values too (a dense weight with a sparse gradient: gluon's
+// Embedding(sparse_grad=True) under Trainer). The merge is the same; the update target, its state
+// and the callback's `local` are then the key's whole dense weight on `home`, which has the layout
+// of a table holding every row. Without an updater the key's value becomes the merged row_sparse
+// array (kvstore_local.h:237-243) until a dense push makes it dense again.
 void KVStore::PushRowSparse(KeyEntry& e, const std::vector<NDArray>& srcs_in) {
-  KV_CHECK_EQ(e.stype, kRowSparseStorage)
-      << "key " << e.key << " was initialised dense but a row_sparse value was pushed";
-  KV_CHECK_EQ(e.dtype, kFloat32) << "row_sparse keys are float32 on this path";
+  const bool dense_key = e.stype == kDefaultStorage;
+  // every refusal comes before anything is enqueued: value and state stay as they were
+  KV_CHECK_EQ(e.dtype, kFloat32) << (dense_key ? "row_sparse values pushed to a dense key are float32 on this path"
+                                               : "row_sparse keys are float32 on this path");
   KV_CHECK(srcs_in.size() <= static_cast<size_t>(kMaxSrc));
+  for (auto& s : srcs_in) {
+    KV_CHECK(s.shape() == e.shape) << "push: shape mismatch for row_sparse key " << e.key;
+    KV_CHECK_EQ(s.dtype(), e.dtype) << "push: dtype mismatch for key " << e.key;
+  }
+  if (dense_key) {
+    KV_CHECK(!dist_) << "key " << e.key << " was initialised dense: the one-rank-per-GPU store takes "
+                     << "dense values for it only";
+    KV_CHECK(!nccl_type_) << "kvstore 'nccl' does not take row_sparse values (src/kvstore/kvstore_nccl.h:93-94)";
+    KV_CHECK(!opt_.enabled || opt_.kind == kOptSGD || opt_.kind == kOptAdam)
+        << "the store's fused optimizer takes row_sparse values for sgd and adam only";
+  }
   Engine* eng = Engine::Get();
   if (dist_ && e.home < 0) e.home = PeerGroup::Get()->dev();
+  if (dense_key && e.striped) EnsureWhole(e, devset_[0]);   // state included; dense pushes restripe it
   if (e.home < 0) {
     int pick = 0;
     for (auto& s : srcs_in) {
       if (s.on_gpu()) { pick = s.dev(); break; }
     }
-    e.home = pick;
+    if (dense_key) EnsureOnDevice(e, pick); else e.home = pick;
   }
   const int home = e.home;
-  if (!e.rsp.on_gpu()) e.rsp = e.rsp.Copy(Context::GPU(home));
+  const bool callback = updater_ != nullptr && !opt_.enabled;
+  if (dense_key && (opt_.enabled || callback)) DensifyValue(e);   // the update reads the dense weight
+  if (!dense_key && !e.rsp.on_gpu()) e.rsp = e.rsp.Copy(Context::GPU(home));
+  // the update target: the row_sparse table, or the dense weight
+  const NDArray W = dense_key ? e.dev[home].w : e.rsp;
   std::vector<NDArray> srcs;
   std::vector<int> parts{home};
   for (auto& s : srcs_in) {
-    KV_CHECK(s.shape() == e.shape) << "push: shape mismatch for row_sparse key " << e.key;
-    KV_CHECK_EQ(s.dtype(), e.dtype) << "push: dtype mismatch for key " << e.key;
     if (!s.on_gpu()) {
       srcs.push_back(s.Copy(Context::GPU(home)));
     } else {
@@ -139,14 +159,14 @@ void KVStore::PushRowSparse(KeyEntry& e, const std::vector<NDArray>& srcs_in) {
   const RspSources S = LocalSources(srcs);
   int64_t total = S.start[S.nsrc];
   NDArray merged = NDArray::RowSparse(e.shape, Context::GPU(home), e.dtype);
-  const int64_t row_len = static_cast<int64_t>(e.rsp.RowLength());
+  const int64_t row_len = static_cast<int64_t>(W.RowLength());
   const bool on_store = opt_.enabled && (opt_.kind == kOptSGD || opt_.kind == kOptAdam);
   // lazy: the optimizer step is fused into the row-sum kernel. standard (lazy_update=False): the
   // merged gradient is materialised, then every row of the table is updated (RunRspStdUpdate).
   const bool fused = on_store && opt_.lazy_update;
   RspUpdateLaunch U;
   if (on_store) {
-    KV_CHECK(!e.rsp_devs.empty() || e.rsp_group || e.rsp.nnr() == e.shape[0])
+    KV_CHECK(dense_key || !e.rsp_devs.empty() || e.rsp_group || e.rsp.nnr() == e.shape[0])
         << "key " << e.key << ": the stored row_sparse weight must hold every row for sparse "
         << "optimizer updates (initialise it from a dense weight, as gluon does)";
     // Optimizer._update_count, then SGD._update_impl's non-aggregated branch / Adam.update
@@ -182,7 +202,7 @@ void KVStore::PushRowSparse(KeyEntry& e, const std::vector<NDArray>& srcs_in) {
     U.wd = ScalarParam(wdd);
     U.rescale = ScalarParam(opt_.rescale);
     U.clip = opt_.clip != 0.0 ? ScalarParam(opt_.clip) : -1.f;
-    U.w = sharded_now ? nullptr : static_cast<float*>(e.rsp.data());
+    U.w = sharded_now ? nullptr : static_cast<float*>(W.data());
     U.s1 = s.s1.is_none() ? nullptr : static_cast<float*>(s.s1.data());
     U.s2 = s.s2.is_none() ? nullptr : static_cast<float*>(s.s2.data());
     U.row_len = row_len;
@@ -198,14 +218,14 @@ void KVStore::PushRowSparse(KeyEntry& e, const std::vector<NDArray>& srcs_in) {
     merged = MergeRowSparseGroup(e, srcs[0]);
     total = 0;   // the merge is done: skip the single-process union below
   }
-  if (fused && total > 0 && parts.size() >= 2 && std::getenv("B200KV_RSP_SHARD_OFF") == nullptr) {
+  if (fused && !dense_key && total > 0 && parts.size() >= 2 && std::getenv("B200KV_RSP_SHARD_OFF") == nullptr) {
     // sources on several GPUs: every GPU merges and updates its own row range of the table
     if (PushRowSparseSharded(e, srcs, parts, U)) return;
   }
   if (!e.rsp_devs.empty()) UnshardRsp(e);
   if (fused) {   // (re)bind the update to the whole table on `home`
     DevState& hs = e.dev[home];
-    U.w = static_cast<float*>(e.rsp.data());
+    U.w = static_cast<float*>(W.data());
     U.s1 = hs.s1.is_none() ? nullptr : static_cast<float*>(hs.s1.data());
     U.s2 = hs.s2.is_none() ? nullptr : static_cast<float*>(hs.s2.data());
   }
@@ -218,7 +238,7 @@ void KVStore::PushRowSparse(KeyEntry& e, const std::vector<NDArray>& srcs_in) {
     // the sources are read on their own lanes; the joins order those lanes around the home lane's work
     for (auto& s : srcs) eng->BeginRead(s.dev(), *s.var());
     LaneOp op(home);
-    if (fused) op.Write(e.rsp).Write(e.dev[home].s1).Write(e.dev[home].s2);
+    if (fused) op.Write(W).Write(e.dev[home].s1).Write(e.dev[home].s2);
     else op.Write(merged);
     op.Write(d_nnr).Write(ws);
     if (parts.size() > 1) eng->JoinStreams(parts);
@@ -242,12 +262,12 @@ void KVStore::PushRowSparse(KeyEntry& e, const std::vector<NDArray>& srcs_in) {
   if (fused) return;
   if (on_store) {
     DevState& ds = e.dev[home];
-    RunRspStdUpdate(e.rsp, merged, ds.s1, ds.s2, U);
+    RunRspStdUpdate(W, merged, ds.s1, ds.s2, U);
     return;
   }
-  if (updater_ != nullptr && !opt_.enabled) {
+  if (callback) {
     NDArray* recv_h = new NDArray(merged);
-    NDArray* local_h = new NDArray(e.rsp);
+    NDArray* local_h = new NDArray(dense_key ? W.Reshaped(e.shape) : W);
     if (key_type_ == 0 && str_updater_ != nullptr) {
       str_updater_(reverse_str_key_dict_[e.key].c_str(), recv_h, local_h, updater_handle_);
     } else {
@@ -256,6 +276,10 @@ void KVStore::PushRowSparse(KeyEntry& e, const std::vector<NDArray>& srcs_in) {
     return;
   }
   e.rsp = merged;  // no updater: local = merged (kvstore_local.h:237-243)
+  if (e.vstype != kRowSparseStorage) {
+    e.vstype = kRowSparseStorage;
+    ++layout_epoch_;   // cached dense pulls of the key must not replay
+  }
 }
 
 // row_sparse_pull (KVStoreLocal::PullRowSparseImpl kvstore_local.h:263-283, Unique :428-472,
@@ -284,7 +308,7 @@ void KVStore::PullRowSparse(const std::vector<int>& keys, const std::vector<NDAr
   std::map<int, std::vector<size_t>> by_home;  // owner GPU -> triples, in key order
   for (size_t i : order) {
     KeyEntry& e = Entry(keys[i]);
-    KV_CHECK_EQ(e.stype, kRowSparseStorage) << "PullRowSparse expects row_sparse src NDArray";
+    KV_CHECK_EQ(e.vstype, kRowSparseStorage) << "PullRowSparse expects row_sparse src NDArray";
     const NDArray& out = outs[i];
     if (e.home < 0) e.home = out.on_gpu() ? out.dev() : (row_ids[i].on_gpu() ? row_ids[i].dev() : 0);
     const bool sharded = !e.rsp_devs.empty() || e.rsp_group;
@@ -511,6 +535,73 @@ void CastStorageCopy(const NDArray& from_in, const NDArray& to) {
     op.Issue();
   }
   if (!target.SameStorage(to)) CopyFromTo(target, to);
+}
+
+void BroadcastRspValue(const NDArray& src, const std::vector<NDArray>& outs) {
+  KV_CHECK(src.on_gpu() && src.stype() == kRowSparseStorage);
+  // the checks CopyFromTo and CastStorageCopy make, for every out before any is written
+  for (auto& o : outs) {
+    KV_CHECK(!o.is_none()) << "copy of an empty NDArray";
+    KV_CHECK_EQ(src.dtype(), o.dtype()) << "CopyFromTo: dtype mismatch";
+    if (o.stype() == kDefaultStorage) {
+      KV_CHECK_EQ(src.dtype(), kFloat32) << "storage casts are float32 on this path";
+      KV_CHECK(src.shape() == o.shape()) << "CopyFromTo: operands shape mismatch";
+    } else {
+      KV_CHECK_EQ(o.stype(), kRowSparseStorage) << "CopyFromTo: unsupported storage type " << o.stype();
+      KV_CHECK(src.shape() == o.shape()) << "CopyFromTo: row_sparse shape mismatch";
+    }
+  }
+  Engine* eng = Engine::Get();
+  const int home = src.dev();
+  const int64_t nnr = src.storage_initialized() ? src.nnr() : 0;
+  for (size_t b = 0; b < outs.size(); b += kMaxDst) {
+    const size_t e = std::min(outs.size(), b + kMaxDst);
+    RspBroadcastLaunch L;
+    L.src_idx = nnr > 0 ? src.row_ids() : nullptr;
+    L.src_val = nnr > 0 ? src.data() : nullptr;
+    L.nnr = nnr;
+    L.rows = src.shape()[0];
+    L.row_bytes = static_cast<int64_t>(src.RowLength() * DTypeSize(src.dtype()));
+    std::vector<NDArray> targets, staged;   // staged[i]: host out of targets[i], or none
+    std::vector<int> parts{home};
+    for (size_t i = b; i < e; ++i) {
+      const NDArray& o = outs[i];
+      if (o.SameStorage(src)) continue;     // self-copy (ndarray.cc:1199-1203)
+      const bool rsp = o.stype() == kRowSparseStorage;
+      if (rsp && nnr == 0) {                // CopyFromToRspImpl of an all-zero value
+        eng->WaitToWrite(*o.var());
+        o.SetNnr(0);
+        continue;
+      }
+      NDArray t = o.on_gpu() ? o
+                 : rsp ? NDArray::RowSparse(o.shape(), Context::GPU(home), o.dtype())
+                       : NDArray(o.shape(), Context::GPU(home), o.dtype());
+      if (rsp) {
+        if (!t.RowsFit(nnr)) eng->WaitToWrite(*t.var());  // buffers get re-allocated
+        t.CheckAndAllocRows(nnr);
+        L.rsp_idx[L.n_rsp] = t.row_ids();
+        L.rsp_val[L.n_rsp++] = t.data();
+      } else {
+        L.dns[L.n_dns++] = t.data();
+      }
+      if (std::find(parts.begin(), parts.end(), t.dev()) == parts.end()) parts.push_back(t.dev());
+      targets.push_back(t);
+      staged.push_back(o.on_gpu() ? NDArray() : o);
+    }
+    if (targets.empty()) continue;
+    eng->RequirePeerAccess(parts);
+    LaneOp op(home);
+    op.Read(src);
+    for (auto& t : targets) op.Write(t);
+    LaunchRspBroadcast(L, op.stream());
+    eng->CountLaunch("rsp_broadcast", static_cast<uint64_t>(nnr) * L.row_bytes +
+                                          static_cast<uint64_t>(L.n_rsp) * nnr * (L.row_bytes + 8) +
+                                          static_cast<uint64_t>(L.n_dns) * L.rows * L.row_bytes);
+    op.Issue();
+    for (size_t k = 0; k < targets.size(); ++k) {
+      if (!staged[k].is_none()) CopyFromTo(targets[k], staged[k]);
+    }
+  }
 }
 
 // =================================================================================================

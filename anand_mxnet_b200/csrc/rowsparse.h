@@ -17,4 +17,10 @@ void RunRspStdUpdate(const NDArray& w, const NDArray& g, const NDArray& s1, cons
 // rows over zeros. float32 only; the cast runs on a GPU (the source's, else the target's).
 void CastStorageCopy(const NDArray& from, const NDArray& to);
 
+// CopyFromTo(src, out) for every out at once (a whole-value pull of a row_sparse value, comm.h:
+// 598-616): ONE launch on src's GPU writes every target, row_sparse outs get the ids and rows,
+// dense outs every table row (stored row or zeros). Outs on other GPUs are written by peer stores,
+// host outs through a staging array. Every out is checked before anything is enqueued.
+void BroadcastRspValue(const NDArray& src, const std::vector<NDArray>& outs);
+
 }  // namespace b200kv

@@ -981,6 +981,74 @@ retain_kernel(const RetainItem* items, int nitems, int64_t total, int id_bits, c
   }
 }
 
+// ---------------------------------------------------------------------------------------------
+// whole-value pull of a row_sparse value: every target in one pass (see LaunchRspBroadcast)
+
+// One row to every target: `src` (null: a row the value does not hold) is read once, in units of
+// T, 4 units in flight per lane; dense targets get it (or zeros) at table row `row`, row_sparse
+// targets at position `pos` (< 0: none).
+template <typename T>
+__device__ __forceinline__ void bcast_row(const RspBroadcastLaunch& p, const T* src, int64_t row, int64_t pos,
+                                          int lane) {
+  const int64_t nu = p.row_bytes / static_cast<int64_t>(sizeof(T));
+  for (int64_t v0 = lane; v0 < nu; v0 += 128) {
+    T x[4];
+#pragma unroll
+    for (int u = 0; u < 4; ++u) {
+      const int64_t v = v0 + 32 * u;
+      x[u] = (src != nullptr && v < nu) ? src[v] : T{};
+    }
+    for (int t = 0; t < p.n_dns; ++t) {
+      T* out = reinterpret_cast<T*>(static_cast<char*>(p.dns[t]) + row * p.row_bytes);
+#pragma unroll
+      for (int u = 0; u < 4; ++u) {
+        if (v0 + 32 * u < nu) out[v0 + 32 * u] = x[u];
+      }
+    }
+    if (pos >= 0) {
+      for (int t = 0; t < p.n_rsp; ++t) {
+        T* out = reinterpret_cast<T*>(static_cast<char*>(p.rsp_val[t]) + pos * p.row_bytes);
+#pragma unroll
+        for (int u = 0; u < 4; ++u) {
+          if (v0 + 32 * u < nu) out[v0 + 32 * u] = x[u];
+        }
+      }
+    }
+  }
+  if (pos >= 0 && lane < p.n_rsp) p.rsp_idx[lane][pos] = row;
+}
+
+// Persistent warps, each over a contiguous range of the domain: the table's rows when a dense
+// target is present (one lower bound finds the range's first stored row, then the warp walks the
+// ids alongside the rows), else the stored rows. The id of the next stored row is loaded before
+// the current row is copied, so the copy never waits for it.
+template <typename T>
+__global__ void __launch_bounds__(kWarpsPerBlock * 32)
+rsp_broadcast_kernel(const __grid_constant__ RspBroadcastLaunch p) {
+  const int lane = threadIdx.x & 31;
+  const int64_t nwarps = static_cast<int64_t>(gridDim.x) * kWarpsPerBlock;
+  const int64_t warp = static_cast<int64_t>(blockIdx.x) * kWarpsPerBlock + (threadIdx.x >> 5);
+  const bool dense = p.n_dns > 0;
+  const int64_t domain = dense ? p.rows : p.nnr;
+  const int64_t per = (domain + nwarps - 1) / nwarps;
+  const int64_t lo = warp * per, hi = min(domain, lo + per);
+  if (lo >= hi) return;
+  const T* val = static_cast<const T*>(p.src_val);
+  const int64_t row_units = p.row_bytes / static_cast<int64_t>(sizeof(T));
+  int64_t pos = dense ? warp_lower_bound(p.src_idx, p.nnr, lo, lane) : lo;
+  int64_t next = pos < p.nnr ? p.src_idx[pos] : INT64_MAX;
+  for (int64_t i = lo; i < hi; ++i) {
+    const int64_t row = dense ? i : next;
+    if (row == next) {
+      const int64_t cur = pos++;
+      next = pos < p.nnr ? p.src_idx[pos] : INT64_MAX;
+      bcast_row<T>(p, val + cur * row_units, row, cur, lane);
+    } else {
+      bcast_row<T>(p, static_cast<const T*>(nullptr), row, -1, lane);
+    }
+  }
+}
+
 struct RetainLayout {
   size_t items, comp, sorted, uniq, count, temp, temp_bytes, total;
   // bitmap unique (id_bits > 0 and the table is short enough): bitmap + prefix per item live in the
@@ -1276,6 +1344,25 @@ void LaunchRspScatterRows(const int64_t* idx, const float* val, int64_t nnr, int
   if (nnr <= 0 || row_len <= 0) return;
   const int blocks = static_cast<int>((nnr + kWarpsPerBlock - 1) / kWarpsPerBlock);
   rsp_scatter_rows_kernel<<<blocks, kWarpsPerBlock * 32, 0, stream>>>(idx, val, nnr, row_len, dense);
+  KV_CUDA(cudaGetLastError());
+}
+
+void LaunchRspBroadcast(const RspBroadcastLaunch& p, cudaStream_t stream) {
+  const int64_t domain = p.n_dns > 0 ? p.rows : p.nnr;
+  if (domain <= 0 || p.row_bytes <= 0 || p.n_dns + p.n_rsp == 0) return;
+  KV_CHECK(p.n_dns <= kMaxDst && p.n_rsp <= kMaxDst);
+  uintptr_t bits = reinterpret_cast<uintptr_t>(p.src_val) | static_cast<uintptr_t>(p.row_bytes);
+  for (int t = 0; t < p.n_dns; ++t) bits |= reinterpret_cast<uintptr_t>(p.dns[t]);
+  for (int t = 0; t < p.n_rsp; ++t) bits |= reinterpret_cast<uintptr_t>(p.rsp_val[t]);
+  const int blocks = static_cast<int>(std::min<int64_t>((domain + kWarpsPerBlock - 1) / kWarpsPerBlock, kNumSMs * 8));
+  const int threads = kWarpsPerBlock * 32;
+  if ((bits & 15) == 0) {
+    rsp_broadcast_kernel<uint4><<<blocks, threads, 0, stream>>>(p);
+  } else if ((bits & 3) == 0) {
+    rsp_broadcast_kernel<uint32_t><<<blocks, threads, 0, stream>>>(p);
+  } else {
+    rsp_broadcast_kernel<uint8_t><<<blocks, threads, 0, stream>>>(p);
+  }
   KV_CUDA(cudaGetLastError());
 }
 
