@@ -262,6 +262,7 @@ int MXNDArrayGetData(NDArrayHandle handle, void** out_pdata) {
   API_BEGIN();
   KVStore::FlushAll();  // the caller is about to look at the memory
   NDArray& a = ND(handle);
+  a.Escape();
   *out_pdata = a.is_none() ? nullptr : a.data();
   API_END();
 }
@@ -409,6 +410,7 @@ int MXNDArrayToDLPack(NDArrayHandle handle, DLManagedTensorHandle* out_dlpack) {
   KVStore::FlushAll();  // queued (bucketed) KVStore calls run before anything observes arrays
   NDArray& a = ND(handle);
   KV_CHECK_EQ(a.stype(), kDefaultStorage) << "only dense arrays export to DLPack";
+  a.Escape();
   struct Holder {
     NDArray arr;
     std::vector<int64_t> shape;

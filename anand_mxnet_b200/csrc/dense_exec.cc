@@ -380,12 +380,23 @@ void KVStore::RunPrepared(Prepared& P) {
   const bool multi = P.parts.size() > 1;
   const int host_lane = P.owners[0];  // kernel-visible host operands are touched by the owners' kernels
   auto lane_of = [&](const NDArray& a) { return a.on_gpu() ? a.dev() : host_lane; };
+  // arrays the kernel reads besides the state: the sources, and `w_in` when the call moves the
+  // stored value between the store's buffer and a pull anchor
+  auto for_reads = [](const DenseOp& op, auto&& f) {
+    for (auto& s : op.srcs) f(s);
+    if (!op.w_in.is_none()) f(op.w_in);
+  };
   for (auto& op : P.ops) {
-    for (auto& s : op.srcs) eng->BeginRead(lane_of(s), *s.var());
+    for_reads(op, [&](const NDArray& s) { eng->BeginRead(lane_of(s), *s.var()); });
     for (auto& o : op.outs) eng->BeginWrite(lane_of(o), *o.var());
     for (int d : P.owners) {
       DevState& s = op.e->dev[d];
-      if (P.is_push) eng->BeginWrite(d, *s.w.var()); else eng->BeginRead(d, *s.w.var());
+      if (P.is_push) {
+        Engine::AnchorWriteScope anchored_step;  // `w` may be the key's pull anchor
+        eng->BeginWrite(d, *s.w.var());
+      } else {
+        eng->BeginRead(d, *s.w.var());
+      }
     }
   }
   if (multi) eng->JoinStreams(P.parts);
@@ -451,7 +462,7 @@ void KVStore::RunPrepared(Prepared& P) {
   uint64_t seq[kMaxDevices] = {0};
   for (int d : P.parts) seq[d] = eng->Issue(d);
   for (auto& op : P.ops) {
-    for (auto& s : op.srcs) eng->MarkRead(lane_of(s), seq[lane_of(s)], s.var());
+    for_reads(op, [&](const NDArray& s) { eng->MarkRead(lane_of(s), seq[lane_of(s)], s.var()); });
     for (auto& o : op.outs) eng->MarkWrite(lane_of(o), seq[lane_of(o)], o.var());
     for (int d : P.owners) {
       DevState& s = op.e->dev[d];

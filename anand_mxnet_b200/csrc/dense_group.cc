@@ -316,6 +316,7 @@ std::shared_ptr<Plan> KVStore::GetPlanGroup(const std::vector<DenseOp>& ops, int
     DevState& s = e.dev[dev];
     const bool use_state = opt_kind == kOptSGD || opt_kind == kOptAdam;
     K.w = s.w.data();
+    K.w_in = K.w;
     K.w32 = (use_state && !s.w32.is_none()) ? static_cast<float*>(s.w32.data()) : nullptr;
     K.s1 = (use_state && !s.s1.is_none()) ? static_cast<float*>(s.s1.data()) : nullptr;
     K.s2 = (opt_kind == kOptAdam && !s.s2.is_none()) ? static_cast<float*>(s.s2.data()) : nullptr;

@@ -138,7 +138,7 @@ __device__ __forceinline__ void process(const KeyDesc& k, uint32_t off, uint32_t
         if (mp) {
           IO<float, V>::ld(k.w32 + base[u], wv[u]);
         } else {
-          IO<T, V>::ld(static_cast<const T*>(k.w) + base[u], wv[u]);
+          IO<T, V>::ld(static_cast<const T*>(k.w_in) + base[u], wv[u]);
         }
         if ((OPT == kOptSGD && has_mom) || OPT == kOptAdam) IO<float, V>::ld(k.s1 + base[u], s1[u]);
         if (OPT == kOptAdam) IO<float, V>::ld(k.s2 + base[u], s2[u]);
@@ -193,7 +193,7 @@ __device__ __forceinline__ void process(const KeyDesc& k, uint32_t off, uint32_t
   } else {
 #pragma unroll
     for (int u = 0; u < U; ++u) {
-      if (on[u]) IO<T, V>::ld(static_cast<const T*>(k.w) + base[u], acc[u]);
+      if (on[u]) IO<T, V>::ld(static_cast<const T*>(k.w_in) + base[u], acc[u]);
     }
   }
   // ---- broadcast to every pull target (peer stores ride NVLink)
@@ -480,7 +480,7 @@ __global__ void __launch_bounds__(kThreads) dense_plain_kernel(const KernelArgs 
         }
         static_cast<T*>(sk.w)[i] = acc;
       } else {
-        acc = static_cast<const T*>(sk.w)[i];
+        acc = static_cast<const T*>(sk.w_in)[i];
       }
       for (int o = 0; o < n_out; ++o) static_cast<T*>(sk.out[o])[i] = acc;
     }

@@ -106,6 +106,7 @@ void Engine::HostWait(Tag t) {
 void Engine::BeginRead(int sid, const Var& v) { StreamWait(sid, v.writer); }
 
 void Engine::BeginWrite(int sid, const Var& v) {
+  if (v.anchor != nullptr && anchor_writes_ok == 0) detach_anchor(const_cast<Var*>(&v));
   StreamWait(sid, v.writer);
   if (v.has_readers) {
     for (int e = 0; e < kMaxStreams; ++e) {
@@ -145,6 +146,7 @@ void Engine::WaitToRead(const Var& v) {
 }
 
 void Engine::WaitToWrite(const Var& v) {
+  if (v.anchor != nullptr && anchor_writes_ok == 0) detach_anchor(const_cast<Var*>(&v));
   HostWait(v.writer);
   if (v.has_readers) {
     for (int e = 0; e < kMaxStreams; ++e) {
@@ -286,6 +288,7 @@ void Engine::Free(int dev, void* p, size_t bytes, const Var* last_use) {
   if (last_use != nullptr) {
     b.pending = *last_use;
     b.pending.err.reset();
+    b.pending.anchor = nullptr;
   } else {
     b.pending.writer = Tag{dev, lanes_[dev].issued};
   }

@@ -43,6 +43,8 @@ struct Var {
   // deferred failure of the asynchronous operation that last wrote the array: re-thrown by the
   // next wait on it (src/engine/threaded_engine.h:380-387, ThrowException / var_exception)
   std::shared_ptr<std::string> err;
+  // the store that keeps a key's value in this array (a pull anchor, kvstore.h), or null
+  void* anchor = nullptr;
 };
 
 class Engine {
@@ -62,6 +64,16 @@ class Engine {
   // An op on one lane uses LaneOp (ndarray.h), which names each array once for both steps.
   void BeginRead(int sid, const Var& v);   // lane waits for v's writer
   void BeginWrite(int sid, const Var& v);  // ... and for every reader
+  // Copy-on-write of pull anchors: a write declared on an anchor (BeginWrite, WaitToWrite) first
+  // calls detach_anchor, which hands the value back to the store -- a copy enqueued after the
+  // anchor's last writer, so ahead of the new write. The store's own fused step writes its anchors
+  // inside an AnchorWriteScope.
+  void (*detach_anchor)(Var* v) = nullptr;
+  int anchor_writes_ok = 0;
+  struct AnchorWriteScope {
+    AnchorWriteScope() { ++Get()->anchor_writes_ok; }
+    ~AnchorWriteScope() { --Get()->anchor_writes_ok; }
+  };
   uint64_t Issue(int sid);
   void MarkRead(int sid, uint64_t seq, Var* v);
   void MarkWrite(int sid, uint64_t seq, Var* v);

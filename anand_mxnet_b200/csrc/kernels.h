@@ -34,7 +34,10 @@ enum SumOrder : int {
 struct alignas(16) KeyDesc {
   const void* src[kMaxSrc];  // gradient of every source (local or peer-mapped), dtype = key dtype
   void* out[kMaxDst];        // pull targets (local or peer-mapped), dtype = key dtype
-  void* w;                   // stored value on this device (key dtype)
+  void* w;                   // stored value on this device, written (key dtype)
+  // stored value on this device, read: w itself, except on the step that moves the value between
+  // the store's own buffer and a pull anchor (kvstore.h, DevState)
+  const void* w_in;
   float* w32;                // fp32 master weights (16-bit keys under multi_precision) or null
   float* s1;                 // momentum / Adam mean (fp32) or null
   float* s2;                 // Adam var (fp32) or null
@@ -49,8 +52,8 @@ struct alignas(16) KeyDesc {
   // out[kMaxDst-2], out[kMaxDst-1] the multicast addresses of the pull targets (one multimem.st
   // reaches every rank). The unicast src[]/out[] entries stay valid for the scalar tail path.
   uint32_t nvls;
-  uint32_t pad_[2];
 };
+static_assert(sizeof(KeyDesc) == 320, "KeyDesc: 20 uint4 words");
 
 struct alignas(16) ChunkDesc {
   uint32_t key;  // index into the KeyDesc table

@@ -42,8 +42,20 @@ struct OptConfig {
   std::unordered_map<int, int> count;  // Optimizer._index_update_count
 };
 
+// Pull anchors. After a pushpull writes a key's new value into a pull target `out`, the store and
+// the caller hold the same bits. The value may then simply LIVE in `out` (the key's anchor): the
+// next step reads gradient, `out` and state and writes `out` and state -- the copy in the store's
+// own buffer is neither written nor read again (20 instead of 24 bytes per element for SGD with
+// momentum). Invariant: the anchor holds the stored value bit for bit, or the key has no anchor.
+// Only whole, never-escaped GPU arrays on the key's home GPU anchor, in a single-process store, for
+// unstriped float32 keys and float16 / bfloat16 keys not under SGD / Adam (which keep fp32 master
+// weights), and only an `out` that no other operand of the call touches. Any other write to the
+// anchor's storage (engine.h, detach_anchor) first copies the value back into `own`.
+// B200KV_PULL_ANCHOR=0 (read whenever a call is planned) forms no anchor and ends existing ones.
 struct DevState {
-  NDArray w;    // stored value replica (key dtype)
+  NDArray w;    // stored value replica (key dtype): `own`, or a view of the anchor
+  NDArray own;  // the store's buffer while `w` is an anchor (kept, so a detach never allocates)
+  bool anchored = false;
   NDArray w32;  // fp32 master (16-bit keys + multi_precision)
   NDArray s1;   // momentum / Adam mean
   NDArray s2;   // Adam var
@@ -88,6 +100,9 @@ struct DenseOp {
   KeyEntry* e = nullptr;
   std::vector<NDArray> srcs;  // empty: pull only
   std::vector<NDArray> outs;  // empty: push only
+  // where the kernel reads the stored value when the call moves it between `own` and an anchor
+  // (none: the stored value `w` of the owner)
+  NDArray w_in;
 };
 
 // Device-resident descriptor tables of one fused launch, cached by call signature.
@@ -199,6 +214,9 @@ class KVStore {
   void SetBucketBytes(size_t n);
   void Flush();
   static void FlushAll();
+  // engine.h detach_anchor: a write to the anchor `v` of one of this store's keys is about to be
+  // declared
+  void DetachVar(Var* v);
   std::string DescribePlan(const std::vector<int>& keys, int num_devices);
 
  private:
@@ -225,6 +243,19 @@ class KVStore {
   bool RunCachedCall(const std::vector<uint64_t>& sig);
   void StoreCachedCall(const std::vector<uint64_t>& sig, std::vector<Prepared>&& launches);
   void ExecCallbackPush(KeyEntry& e, const std::vector<NDArray>& srcs);
+  // pull anchors (DevState): settled for a call before it is planned; true when one formed or ended.
+  // `moves` records what formed or ended, so that a call refused while it is planned -- before any
+  // launch -- leaves every value where it was (UndoAnchorMoves).
+  struct AnchorMove {
+    KeyEntry* e;
+    NDArray anchor;
+    bool formed;
+  };
+  bool ResolveAnchors(std::vector<DenseOp>* fused, std::vector<DenseOp>* pulls, std::vector<AnchorMove>* moves);
+  void UndoAnchorMoves(const std::vector<AnchorMove>& moves);
+  bool AnchorEligible(const KeyEntry& e) const;
+  void DetachAnchor(KeyEntry& e);                       // the value back into `own` (a copy)
+  std::unordered_map<const Var*, KeyEntry*> anchors_;
   void DensifyValue(KeyEntry& e);                       // dense key: row_sparse value -> dense weight
   NDArray RowSparseValue(KeyEntry& e, const std::vector<NDArray>& outs);  // whole, on a GPU
   void EnsureOnDevice(KeyEntry& e, int dev);            // HOST -> WHOLE(dev)

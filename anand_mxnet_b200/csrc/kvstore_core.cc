@@ -29,6 +29,8 @@ static bool Is16Bit(int dtype) { return dtype == kFloat16 || dtype == kBfloat16;
 
 static std::set<KVStore*>& LiveStores();  // stores with possibly queued work (FlushAll)
 
+static void DetachAnchorOf(Var* v) { static_cast<KVStore*>(v->anchor)->DetachVar(v); }
+
 // Chunk a key's elements for the device that owns them. A chunk never crosses a chunk boundary of
 // the store-global element space, hence never an ownership stripe. owner_fixed >= 0: the whole key
 // belongs to that slot (WHOLE placement); otherwise stripes rotate over ndev slots.
@@ -95,6 +97,7 @@ KVStore::KVStore(const std::string& type) : type_(type) {
     auto_bucket_bytes_ = static_cast<size_t>(std::max(1, std::atoi(b))) << 20;
   }
   LiveStores().insert(this);
+  Engine::Get()->detach_anchor = &DetachAnchorOf;
 }
 
 KVStore::~KVStore() {
@@ -104,6 +107,8 @@ KVStore::~KVStore() {
     Engine::Get()->WaitAll();
   } catch (...) {
   }
+  // the anchors keep the last value the caller pulled: theirs from now on
+  for (auto& a : anchors_) const_cast<Var*>(a.first)->anchor = nullptr;
 }
 
 void KVStore::SetKeyTypeInt() {
@@ -634,11 +639,19 @@ void KVStore::PushImpl(const std::vector<int>& keys, const std::vector<NDArray>&
     p.outs = ogrouped[i];
     pulls.push_back(p);
   }
+  // a call that anchors or detaches runs launches of its own; the next identical call is cached
+  std::vector<AnchorMove> moves;
+  const bool moved = ResolveAnchors(&fused, &pulls, &moves);
   std::vector<Prepared> launches;
-  PrepareDense(fused, opt_.enabled ? opt_.kind : kOptAssign, true, &launches);
-  PrepareDense(pulls, kOptPullOnly, true, &launches);
+  try {
+    PrepareDense(fused, opt_.enabled ? opt_.kind : kOptAssign, true, &launches);
+    PrepareDense(pulls, kOptPullOnly, true, &launches);
+  } catch (...) {
+    UndoAnchorMoves(moves);  // a refused call leaves every stored value where it was
+    throw;
+  }
   for (auto& p : launches) RunPrepared(p);
-  if (cacheable) StoreCachedCall(sig, std::move(launches));
+  if (cacheable && !moved) StoreCachedCall(sig, std::move(launches));
 }
 
 void KVStore::PullImpl(const std::vector<int>& keys, const std::vector<NDArray>& outs,
@@ -682,6 +695,8 @@ void KVStore::PullImpl(const std::vector<int>& keys, const std::vector<NDArray>&
     p.outs = grouped[i];
     pulls.push_back(p);
   }
+  std::vector<AnchorMove> moves;  // pulls neither form nor end anchors
+  if (ResolveAnchors(nullptr, &pulls, &moves)) cacheable_call = false;
   if (pulls.empty()) return;
   std::vector<Prepared> launches;
   PrepareDense(pulls, kOptPullOnly, true, &launches);
@@ -731,6 +746,7 @@ void KVStore::EnsureStriped(KeyEntry& e) {
   if (e.striped) return;
   KV_CHECK(devset_.size() >= 1);
   if (e.home < 0) EnsureOnDevice(e, devset_[0]);
+  DetachAnchor(e);
   const DevState src = e.dev[e.home];
   for (int d : devset_) {
     if (d == e.home) continue;
@@ -836,6 +852,156 @@ NDArray KVStore::StageOut(KeyEntry& e, size_t slot, const NDArray&, int dev) {
 }
 
 // =================================================================================================
+// pull anchors (kvstore.h, DevState)
+// =================================================================================================
+bool KVStore::AnchorEligible(const KeyEntry& e) const {
+  if (dist_ || e.striped || e.home < 0 || e.stype != kDefaultStorage || e.vstype != kDefaultStorage) return false;
+  if (e.dtype != kFloat32 && !Is16Bit(e.dtype)) return false;
+  // 16-bit keys under SGD / Adam keep fp32 master weights (or the call is refused without them)
+  if (Is16Bit(e.dtype) && opt_.enabled && (opt_.kind == kOptSGD || opt_.kind == kOptAdam)) return false;
+  auto it = e.dev.find(e.home);
+  return it != e.dev.end() && !it->second.w.is_none() && it->second.w32.is_none();
+}
+
+// The anchor of `s` ends: `w` is the store's own buffer again (whose contents the caller provides).
+static void EndAnchor(DevState& s, std::unordered_map<const Var*, KeyEntry*>* anchors) {
+  s.w.var()->anchor = nullptr;
+  anchors->erase(s.w.var());
+  s.w = s.own;
+  s.anchored = false;
+}
+
+void KVStore::DetachAnchor(KeyEntry& e) {
+  auto it = e.dev.find(e.home);
+  if (e.home < 0 || it == e.dev.end() || !it->second.anchored) return;
+  DevState& s = it->second;
+  const NDArray anchor = s.w;
+  EndAnchor(s, &anchors_);
+  // ordered after the anchor's last writer; a write being declared on the anchor waits for it
+  CopyFromTo(anchor, s.own);
+  ++layout_epoch_;
+}
+
+void KVStore::DetachVar(Var* v) {
+  auto it = anchors_.find(v);
+  if (it == anchors_.end()) {
+    v->anchor = nullptr;
+    return;
+  }
+  DetachAnchor(*it->second);
+}
+
+void KVStore::UndoAnchorMoves(const std::vector<AnchorMove>& moves) {
+  // nothing was launched: a formed anchor was never written and `own` still holds the value; an
+  // ended anchor still holds it
+  for (auto it = moves.rbegin(); it != moves.rend(); ++it) {
+    DevState& s = it->e->dev[it->e->home];
+    if (it->formed) {
+      EndAnchor(s, &anchors_);
+    } else {
+      s.w = it->anchor;
+      s.anchored = true;
+      it->anchor.var()->anchor = this;
+      anchors_[it->anchor.var()] = it->e;
+    }
+  }
+  if (!moves.empty()) ++layout_epoch_;
+}
+
+bool KVStore::ResolveAnchors(std::vector<DenseOp>* fused, std::vector<DenseOp>* pulls,
+                             std::vector<AnchorMove>* moves) {
+  if (dist_) return false;
+  const uint64_t epoch0 = layout_epoch_;
+  // B200KV_PULL_ANCHOR=0, read whenever a call is planned: no anchor forms, and the store's
+  // existing anchors end here
+  const char* env = std::getenv("B200KV_PULL_ANCHOR");
+  const bool form = env == nullptr || env[0] != '0';
+  if (!form && !anchors_.empty()) {
+    std::vector<KeyEntry*> anchored;
+    for (auto& a : anchors_) anchored.push_back(a.second);
+    for (KeyEntry* e : anchored) DetachAnchor(*e);
+  }
+  std::vector<DenseOp>* lists[2] = {fused, pulls};
+  // operands of the whole call per storage: an anchor is an array nothing else in the call touches
+  std::unordered_map<const Storage*, int> uses, out_uses;
+  for (auto* l : lists) {
+    if (l == nullptr) continue;
+    for (auto& op : *l) {
+      for (auto& a : op.srcs) ++uses[a.storage()];
+      for (auto& a : op.outs) {
+        ++uses[a.storage()];
+        ++out_uses[a.storage()];
+      }
+    }
+  }
+  auto sole = [&](const NDArray& a) { return a.WholeStorage() && uses[a.storage()] == 1; };
+  Engine* eng = Engine::Get();
+  for (int li = 0; li < 2; ++li) {
+    if (lists[li] == nullptr) continue;
+    const bool push = li == 0;
+    for (auto& op : *lists[li]) {
+      KeyEntry& e = *op.e;
+      bool local = true;  // a push with a value on another GPU stripes the key
+      for (auto& a : op.srcs) local = local && (!a.on_gpu() || a.dev() == e.home);
+      const bool ok = AnchorEligible(e) && local;
+      if (!ok) DetachAnchor(e);
+      DevState* s = ok ? &e.dev[e.home] : nullptr;
+      // a target that is an anchor stays one only as this key's anchor, touched by nothing else
+      bool into_anchor = false;
+      for (auto& o : op.outs) {
+        if (o.var()->anchor == nullptr) continue;
+        if (s != nullptr && s->anchored && o.SameStorage(s->w) && sole(o)) into_anchor = true;
+        else eng->detach_anchor(o.var());
+      }
+      if (s == nullptr) continue;
+      if (s->anchored) {
+        if (into_anchor) {
+          // the step writes the value where it lives; the anchor is no target of its own
+          op.outs.erase(std::remove_if(op.outs.begin(), op.outs.end(),
+                                       [&](const NDArray& o) { return o.SameStorage(s->w); }),
+                        op.outs.end());
+        } else if (push && out_uses[s->w.storage()] == 0) {
+          // push without a pull into the anchor: the caller's array keeps the value it last
+          // pulled; this step reads the value from it and writes the new one into `own`
+          moves->push_back(AnchorMove{&e, s->w, false});
+          op.w_in = s->w;
+          EndAnchor(*s, &anchors_);
+          ++layout_epoch_;
+        } else if (push) {
+          // ... unless another key of the call writes that array in the same launch
+          DetachAnchor(e);
+        }
+      } else if (push && form) {
+        for (size_t i = 0; i < op.outs.size(); ++i) {
+          const NDArray& o = op.outs[i];
+          if (!o.on_gpu() || o.dev() != e.home || o.external() || o.storage()->escaped || !sole(o) ||
+              o.dtype() != e.dtype || o.Size() != e.size || o.var()->anchor != nullptr) {
+            continue;
+          }
+          // this step reads the value from `own` and writes the new one into the anchor only
+          s->own = s->w;
+          op.w_in = s->own;
+          s->w = o.Reshaped(e.shape);
+          s->anchored = true;
+          o.var()->anchor = this;
+          anchors_[o.var()] = &e;
+          moves->push_back(AnchorMove{&e, s->w, true});
+          op.outs.erase(op.outs.begin() + i);
+          ++layout_epoch_;
+          break;
+        }
+      }
+    }
+  }
+  if (pulls != nullptr) {
+    // a pull into the anchor alone moves no bytes
+    pulls->erase(std::remove_if(pulls->begin(), pulls->end(), [](const DenseOp& op) { return op.outs.empty(); }),
+                 pulls->end());
+  }
+  return layout_epoch_ != epoch0;
+}
+
+// =================================================================================================
 // the fused dense launch
 // =================================================================================================
 static uint64_t HashMix(uint64_t h, uint64_t v) {
@@ -852,6 +1018,7 @@ std::shared_ptr<Plan> KVStore::GetPlan(const std::vector<DenseOp>& ops, int opt_
     for (auto& s : op.srcs) sig = HashMix(sig, reinterpret_cast<uint64_t>(s.data()));
     sig = HashMix(sig, 0xabcdef);
     for (auto& o : op.outs) sig = HashMix(sig, reinterpret_cast<uint64_t>(o.data()));
+    sig = HashMix(sig, reinterpret_cast<uint64_t>(op.w_in.is_none() ? nullptr : op.w_in.data()));
     for (int d : owners) {
       DevState& s = op.e->dev[d];
       sig = HashMix(sig, reinterpret_cast<uint64_t>(s.w.is_none() ? nullptr : s.w.data()));
@@ -890,11 +1057,12 @@ std::shared_ptr<Plan> KVStore::GetPlan(const std::vector<DenseOp>& ops, int opt_
       }
       DevState& s = e.dev[d];
       K.w = s.w.is_none() ? nullptr : s.w.data();
+      K.w_in = op.w_in.is_none() ? K.w : op.w_in.data();
       const bool use_state = opt_kind == kOptSGD || opt_kind == kOptAdam;
       K.w32 = (use_state && !s.w32.is_none()) ? static_cast<float*>(s.w32.data()) : nullptr;
       K.s1 = (use_state && !s.s1.is_none()) ? static_cast<float*>(s.s1.data()) : nullptr;
       K.s2 = (opt_kind == kOptAdam && !s.s2.is_none()) ? static_cast<float*>(s.s2.data()) : nullptr;
-      ok = ok && aligned(K.w) && aligned(K.w32) && aligned(K.s1) && aligned(K.s2);
+      ok = ok && aligned(K.w) && aligned(K.w_in) && aligned(K.w32) && aligned(K.s1) && aligned(K.s2);
       K.n_src = static_cast<int32_t>(op.srcs.size());
       K.n_out = static_cast<int32_t>(op.outs.size());
       K.vec_ok = ok ? 1u : 0u;
@@ -953,6 +1121,7 @@ std::shared_ptr<Plan> KVStore::GetPlan(const std::vector<DenseOp>& ops, int opt_
 // =================================================================================================
 void KVStore::ExecCallbackPush(KeyEntry& e, const std::vector<NDArray>& srcs_in) {
   std::vector<NDArray> srcs = srcs_in;
+  DetachAnchor(e);  // the updater writes the stored value in place
   if (e.striped) EnsureWhole(e, devset_[0]);
   if (e.home < 0) {
     int pick = 0;
@@ -1002,6 +1171,7 @@ void KVStore::ExecCallbackPush(KeyEntry& e, const std::vector<NDArray>& srcs_in)
 // its dense weight -- zeros plus the stored rows -- before anything reads or updates that weight.
 void KVStore::DensifyValue(KeyEntry& e) {
   if (e.vstype == kDefaultStorage) return;
+  DetachAnchor(e);
   BroadcastRspValue(e.rsp, {e.dev[e.home].w});
   e.rsp = NDArray();
   e.vstype = kDefaultStorage;
@@ -1055,6 +1225,7 @@ void KVStore::SetOptimizerState(int key, int state_id, const NDArray& v) {
   }
   KV_CHECK_EQ(v.Size(), e.size) << "optimizer state shape mismatch for key " << key;
   KV_CHECK_EQ(v.dtype(), kFloat32) << "optimizer states are float32";
+  DetachAnchor(e);  // fp32 master weights (state 2) rule an anchor out
   DevState& s = e.dev[dev];
   NDArray* a = state_id == 0 ? &s.s1 : state_id == 1 ? &s.s2 : &s.w32;
   if (a->is_none()) *a = NDArray(e.shape, Context::GPU(dev), kFloat32);

@@ -127,6 +127,17 @@ NDArray NDArray::AuxView() const {
   return v;
 }
 
+void NDArray::Escape() const {
+  if (st_ == nullptr) return;
+  st_->escaped = true;
+  Engine* e = Engine::Get();
+  if (st_->var.anchor == nullptr) return;
+  e->detach_anchor(&st_->var);
+  // whoever writes through the pointer is not ordered by the engine: the copy that took the value
+  // out of this array completes first
+  e->WaitToWrite(st_->var);
+}
+
 NDArray NDArray::Reshaped(const std::vector<int64_t>& shape) const {
   KV_CHECK_EQ(Prod(shape), Size()) << "reshape size mismatch";
   NDArray v = *this;

@@ -33,6 +33,9 @@ struct Storage {
   size_t aux_bytes = 0;
   int64_t nnr = 0;      // row_sparse: rows stored; 0 == storage not initialised == all zeros
   bool external = false;
+  // a raw pointer to the memory went out (MXNDArrayGetData, DLPack export): writes through it are
+  // invisible to the engine, so the array never becomes a pull anchor (kvstore.h)
+  bool escaped = false;
   std::function<void()> deleter;
   Var var;
   ~Storage();
@@ -89,6 +92,10 @@ class NDArray {
   Storage* storage() const { return st_.get(); }
   long use_count() const { return st_.use_count(); }   // holders of the underlying storage
   bool SameStorage(const NDArray& o) const { return st_ == o.st_; }
+  // the view covers its storage's bytes exactly (offset 0, whole allocation)
+  bool WholeStorage() const { return !aux_view_ && byte_offset_ == 0 && ByteSize() == st_->bytes; }
+  // a raw pointer to the memory is handed out: a pull anchor in it ends, and it never becomes one
+  void Escape() const;
 
   void Alloc() const;  // dense: allocate if delayed
   void* data() const;  // dense values / row_sparse value rows

@@ -124,6 +124,7 @@ void RunAdhoc(int opt, std::vector<AdhocKey>& keys, const DenseLaunch& scalars,
       std::memset(&K, 0, sizeof(K));
       AdhocKey& k = keys[i];
       K.w = k.w.data();
+      K.w_in = K.w;
       bool ok = aligned(K.w);
       if (!k.g.is_none()) {
         K.src[0] = k.g.data();

@@ -129,6 +129,7 @@ void KVStore::PushRowSparse(KeyEntry& e, const std::vector<NDArray>& srcs_in) {
         << "the store's fused optimizer takes row_sparse values for sgd and adam only";
   }
   Engine* eng = Engine::Get();
+  DetachAnchor(e);  // the dense weight is updated, or replaced by a row_sparse value, below
   if (dist_ && e.home < 0) e.home = PeerGroup::Get()->dev();
   if (dense_key && e.striped) EnsureWhole(e, devset_[0]);   // state included; dense pushes restripe it
   if (e.home < 0) {
