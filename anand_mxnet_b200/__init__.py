@@ -16,6 +16,7 @@ from .context import Context, cpu, gpu, cpu_pinned
 from . import ndarray
 from . import ndarray as nd
 from . import optimizer
+from . import gluon
 from . import kvstore
 from . import kvstore as kv
 from . import dist

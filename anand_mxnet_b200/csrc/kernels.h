@@ -236,6 +236,30 @@ static_assert(sizeof(AllFiniteArrays) <= 32764, "kernel parameters are limited t
 // dtype: kFloat16, kBfloat16, kFloat32 or kFloat64. Always exactly one launch.
 void LaunchAllFinite(int dtype, AllFiniteArrays& arrays, float* out, cudaStream_t stream);
 
+// _b200kv_clip_global_norm / _b200kv_multi_scale (gluon.utils.clip_global_norm, amp.unscale): float32
+// arrays of one GPU, listed by value like AllFiniteArrays and tiled by bytes the same way. A call
+// with more than kCNMaxArrays arrays goes group by group; nothing here waits on the host.
+constexpr int kCNMaxArrays = 200;
+constexpr int kCNTileBytes = 16384;
+struct ClipNormArrays {
+  float* p[kCNMaxArrays];                    // any 4-byte alignment
+  uint32_t n[kCNMaxArrays];                  // elements (stored rows x row length for row_sparse)
+  uint32_t first_tile[kCNMaxArrays + 1];     // prefix of the tile counts (filled by ClipNormTiles)
+  int32_t count;
+};
+// Fills first_tile; returns the group's number of tiles (0: nothing to launch for it).
+uint32_t ClipNormTiles(ClipNormArrays& arrays);
+// clip_norm_partial: part[0 .. tiles) = each tile's sum of squares. One launch.
+void LaunchClipNormPartial(const ClipNormArrays& arrays, uint32_t tiles, float* part, cudaStream_t stream);
+// clip_norm_fold: ss = part[0] + ... + part[n_part - 1] in one fixed association; *total_norm =
+// sqrtf(ss); *scale = min(max_norm / (total_norm + 1e-8f), 1), and 1 when total_norm is inf / nan.
+void LaunchClipNormFold(const float* part, uint32_t n_part, float max_norm, float* total_norm,
+                        float* scale, cudaStream_t stream);
+// clip_norm_scale: x *= s in place, s = *scale_dev when given, else scale. Returns without reading
+// or writing the arrays when s == 1. One launch.
+void LaunchClipNormScale(const ClipNormArrays& arrays, uint32_t tiles, const float* scale_dev, float scale,
+                         cudaStream_t stream);
+
 // ---- single-tensor optimizer operators of the callback route (update_kernels.cu) ----
 // nag_mom_update, mp_nag_mom_update, signsgd_update, signum_update, rmsprop_update,
 // rmspropalex_update, ftml_update, ftrl_update (optimizer_op-inl.h:1061-1222, 1953-2158, 2344-2431)

@@ -11,6 +11,10 @@
 //   lamb_update_phase1/2, mp_lamb_...     src/operator/optimizer_op.cc:926-1095
 //   _multi_lamb_update, _multi_mp_...     src/operator/contrib/multi_lamb.cc:174-251
 //   all_finite, multi_all_finite          src/operator/contrib/all_finite.cc:42-166
+// Extensions without a reference operator (the reference composes them from NDArray arithmetic):
+//   _b200kv_clip_global_norm              python/mxnet/gluon/utils.py:118-157
+//   _b200kv_multi_scale                   python/mxnet/contrib/amp/amp.py:340-346 (unscale)
+#include <algorithm>
 #include <cmath>
 #include <cstring>
 #include <memory>
@@ -196,6 +200,92 @@ void CheckMP(const NDArray& w, bool mp, const std::string& op) {
   }
 }
 
+// the scalar of the reference's *_scalar operators: std::stod, then one rounding to the array's
+// dtype (elemwise_binary_scalar_op.h:364-365 and its `DType(alpha)`). Not GetF's dmlc::stof.
+float StodF(const Params& p, const char* key, const std::string& op) {
+  const std::string* v = Find(p, key);
+  KV_CHECK(v != nullptr) << "Required parameter " << key << " of " << op << " is missing";
+  try {
+    return static_cast<float>(std::stod(*v));
+  } catch (const std::exception&) {
+    KV_FATAL << op << ": cannot parse " << key << "='" << *v << "'";
+  }
+  return 0.f;
+}
+
+// per-GPU scratch of _b200kv_clip_global_norm: [0] the factor, [1 ...] the tile partials. Every
+// use is on the GPU's compute lane, so consecutive calls share it in stream order; it only grows.
+struct ClipScratch {
+  float* p = nullptr;
+  size_t bytes = 0;
+};
+float* ClipScratchFor(int dev, size_t floats) {
+  static auto* m = new std::unordered_map<int, ClipScratch>();
+  ClipScratch& s = (*m)[dev];
+  const size_t need = floats * sizeof(float);
+  if (s.bytes < need) {
+    Engine* eng = Engine::Get();
+    if (s.p != nullptr) eng->Free(dev, s.p, s.bytes);
+    s.bytes = std::max(need, 2 * s.bytes);
+    s.p = static_cast<float*>(eng->Alloc(dev, s.bytes));
+  }
+  return s.p;
+}
+
+// The operand list both operators share, checked in full before anything is enqueued: float32,
+// dense or row_sparse (its stored rows), one GPU, under 2^32 elements each, no memory listed twice.
+// Returns the groups of <= kCNMaxArrays arrays with their tile counts.
+struct ClipGroup {
+  ClipNormArrays arrays{};
+  uint32_t tiles = 0;
+};
+std::vector<ClipGroup> ClipOperands(const std::string& op, const std::vector<NDArray>& in, const Params& p,
+                                    const char* scalar_key) {
+  for (const auto& kv : p) {
+    KV_CHECK(kv.first == "num_arrays" || kv.first == scalar_key)
+        << "Cannot find argument '" << kv.first << "', Possible Arguments: num_arrays, " << scalar_key;
+  }
+  KV_CHECK(Find(p, "num_arrays") != nullptr) << "Required parameter num_arrays of " << op << " is missing";
+  const int num = GetI(p, "num_arrays", -1);
+  KV_CHECK(num >= 1) << op << ": num_arrays must be at least 1, got " << num;
+  KV_CHECK_EQ(static_cast<int>(in.size()), num) << op << ": expected num_arrays inputs";
+  KV_CHECK(in[0].on_gpu()) << op << " runs on GPU arrays only (no CPU fallback)";
+  const int dev = in[0].dev();
+  std::vector<ClipGroup> groups((num + kCNMaxArrays - 1) / kCNMaxArrays);
+  std::vector<std::pair<uintptr_t, uintptr_t>> spans;  // [begin, end) of every non-empty operand
+  for (int i = 0; i < num; ++i) {
+    const NDArray& a = in[i];
+    KV_CHECK(a.on_gpu() && a.dev() == dev)
+        << op << ": array_" << i << " is not on array_0's GPU; all operands must be on the same GPU "
+        << "(no CPU fallback)";
+    KV_CHECK(a.dtype() == kFloat32)
+        << op << ": array_" << i << " is " << DTypeName(a.dtype())
+        << "; only float32 is served (16-bit gradients are not served yet)";
+    KV_CHECK(a.stype() == kDefaultStorage || a.stype() == kRowSparseStorage)
+        << op << ": array_" << i << " has csr storage; dense and row_sparse arrays are served";
+    const bool rsp = a.stype() == kRowSparseStorage;
+    const uint64_t n = rsp ? static_cast<uint64_t>(a.nnr()) * a.RowLength() : a.Size();
+    KV_CHECK(n < (1ULL << 32)) << op << ": array_" << i << " has 2^32 or more elements";
+    ClipNormArrays& A = groups[i / kCNMaxArrays].arrays;
+    A.n[i % kCNMaxArrays] = static_cast<uint32_t>(n);
+    A.p[i % kCNMaxArrays] = n > 0 ? static_cast<float*>(a.data()) : nullptr;
+    A.count = i % kCNMaxArrays + 1;
+    if (n > 0) {
+      const uintptr_t b = reinterpret_cast<uintptr_t>(a.data());
+      spans.emplace_back(b, b + n * sizeof(float));
+    }
+  }
+  std::sort(spans.begin(), spans.end());
+  for (size_t i = 1; i < spans.size(); ++i) {
+    KV_CHECK(spans[i].first >= spans[i - 1].second)
+        << op << ": two operands share memory (the same storage listed twice); each would be scaled twice";
+  }
+  uint64_t total = 0;
+  for (ClipGroup& g : groups) total += g.tiles = ClipNormTiles(g.arrays);
+  KV_CHECK(total < (1ULL << 31)) << op << ": more than 2^31 tiles of " << kCNTileBytes << " bytes";
+  return groups;
+}
+
 }  // namespace
 
 bool MultiTensorOp(const std::string& n, const std::vector<NDArray>& in, std::vector<NDArray>* outputs,
@@ -266,6 +356,58 @@ bool MultiTensorOp(const std::string& n, const std::vector<NDArray>& in, std::ve
     }
     LaunchAllFinite(dtype, arrays, static_cast<float*>(out.data()), op.stream());
     eng->CountLaunch("all_finite", 0);
+    op.Issue();
+    return true;
+  }
+  // ---------------------------------------------- _b200kv_clip_global_norm, _b200kv_multi_scale
+  if (n == "_b200kv_clip_global_norm") {
+    std::vector<ClipGroup> groups = ClipOperands(n, in, p, "max_norm");
+    const float max_norm = StodF(p, "max_norm", n);
+    KV_CHECK(max_norm > 0.f) << n << ": max_norm must be positive and not nan, got "
+                             << *Find(p, "max_norm");
+    const int dev = in[0].dev();
+    if (!outputs->empty()) {
+      const NDArray& o = (*outputs)[0];
+      KV_CHECK(o.stype() == kDefaultStorage && o.dtype() == kFloat32 && o.shape().size() == 1 &&
+               o.shape()[0] == 1 && o.on_gpu() && o.dev() == dev)
+          << n << ": total_norm must be a dense (1,) float32 array on the inputs' GPU";
+    }
+    NDArray norm = OutOr(outputs, 0, {1}, in[0].ctx(), kFloat32);
+    uint32_t total = 0;
+    for (const ClipGroup& g : groups) total += g.tiles;
+    LaneOp op(dev);
+    for (const NDArray& a : in) op.Write(a);
+    op.Write(norm);
+    Engine* eng = Engine::Get();
+    float* scratch = ClipScratchFor(dev, 1 + static_cast<size_t>(total));
+    uint32_t off = 0;
+    for (const ClipGroup& g : groups) {
+      if (g.tiles == 0) continue;  // only empty arrays: nothing to read
+      LaunchClipNormPartial(g.arrays, g.tiles, scratch + 1 + off, op.stream());
+      eng->CountLaunch("clip_norm_partial", 0);
+      off += g.tiles;
+    }
+    LaunchClipNormFold(scratch + 1, total, max_norm, static_cast<float*>(norm.data()), scratch, op.stream());
+    eng->CountLaunch("clip_norm_fold", 0);
+    for (const ClipGroup& g : groups) {
+      if (g.tiles == 0) continue;
+      LaunchClipNormScale(g.arrays, g.tiles, scratch, 1.f, op.stream());
+      eng->CountLaunch("clip_norm_scale", 0);
+    }
+    op.Issue();
+    return true;
+  }
+  if (n == "_b200kv_multi_scale") {
+    std::vector<ClipGroup> groups = ClipOperands(n, in, p, "scalar");
+    const float scalar = StodF(p, "scalar", n);
+    KV_CHECK(outputs->empty()) << n << " scales its inputs in place and has no output";
+    LaneOp op(in[0].dev());
+    for (const NDArray& a : in) op.Write(a);
+    for (const ClipGroup& g : groups) {
+      if (g.tiles == 0) continue;
+      LaunchClipNormScale(g.arrays, g.tiles, nullptr, scalar, op.stream());
+      Engine::Get()->CountLaunch("clip_norm_scale", 0);
+    }
     op.Issue();
     return true;
   }

@@ -1,7 +1,8 @@
 // multi_tensor_kernels.cu -- the multi-tensor optimizer operators next to the KVStore path
 // (SURVEY 8f-f1): multi_sum_sq, multi_lars, _[mp_]adamw_update, _multi_[mp_]adamw_update,
-// [mp_]lamb_update_phase1/2, _multi_[mp_]lamb_update, and the AMP overflow check
-// [multi_]all_finite (its own kernel and launch list, below).
+// [mp_]lamb_update_phase1/2, _multi_[mp_]lamb_update, the AMP overflow check
+// [multi_]all_finite (its own kernel and launch list, below), and gradient clipping by global
+// norm / the bulk unscale (_b200kv_clip_global_norm, _b200kv_multi_scale: three kernels, below).
 //
 // One launch covers every tensor of the call: a device table of MTTensor descriptors + a list of
 // <= 8192-element chunks (one 256-thread CTA each, 16-byte accesses, streaming loads/stores), the
@@ -427,6 +428,122 @@ __global__ void __launch_bounds__(kAFThreads) all_finite_kernel(const AllFiniteA
   if (__syncthreads_or(bad) && threadIdx.x == 0) *out = 0.0f;
 }
 
+// ---------------------------------------------------------------------------------------------
+// _b200kv_clip_global_norm (python/mxnet/gluon/utils.py:118-157) and _b200kv_multi_scale (the bulk
+// form of amp.unscale, contrib/amp/amp.py:331-346), float32. The array list travels by value and
+// the work is tiled by bytes exactly as for all_finite_kernel: one CTA per kCNTileBytes tile, found
+// by binary search over the first-tile prefix; a 16-byte aligned array moves kCNLoads independent
+// 16-B vectors per thread before any arithmetic, any other base (a[1:]) and the tail go element
+// by element. All loads and stores are default-cached: the scaling pass and then the optimizer
+// read the same gradients next (a streaming hint on the stores has not been measured).
+constexpr int kCNThreads = kThreads;  // block_sum's width
+constexpr int kCNLoads = kCNTileBytes / 16 / kCNThreads;
+constexpr uint32_t kCNTileElems = kCNTileBytes / sizeof(float);
+static_assert(kCNLoads * 16 * kCNThreads == kCNTileBytes, "a tile is whole loads of every thread");
+
+// the last array whose first tile is <= b (arrays without tiles are never found)
+__device__ __forceinline__ int cn_find(const ClipNormArrays& A, uint32_t b) {
+  int lo = 0, hi = A.count - 1;
+  while (lo < hi) {
+    const int mid = (lo + hi + 1) >> 1;
+    if (A.first_tile[mid] <= b) lo = mid; else hi = mid - 1;
+  }
+  return lo;
+}
+
+// part[blockIdx.x] = the tile's sum of x*x: per-thread sequential partial in element order, then
+// block_sum's fixed tree. Padding lanes add +0.0f, which leaves a sum of squares bitwise unchanged.
+__global__ void __launch_bounds__(kCNThreads) clip_norm_partial_kernel(const ClipNormArrays A, float* part) {
+  const uint32_t b = blockIdx.x;
+  const int k = cn_find(A, b);
+  const uint32_t e0 = (b - A.first_tile[k]) * kCNTileElems;
+  const uint32_t len = min(kCNTileElems, A.n[k] - e0);
+  const float* p = A.p[k] + e0;
+  float acc = 0.f;
+  uint32_t scalar_from = 0;
+  if ((reinterpret_cast<uintptr_t>(A.p[k]) & 15) == 0) {
+    const uint32_t nvec = len / 4;
+    const float4* v = reinterpret_cast<const float4*>(p);
+    float4 r[kCNLoads];
+#pragma unroll
+    for (int i = 0; i < kCNLoads; ++i) {
+      const uint32_t j = threadIdx.x + i * kCNThreads;
+      r[i] = j < nvec ? v[j] : make_float4(0.f, 0.f, 0.f, 0.f);
+    }
+#pragma unroll
+    for (int i = 0; i < kCNLoads; ++i) {
+      acc = add(acc, mul(r[i].x, r[i].x));
+      acc = add(acc, mul(r[i].y, r[i].y));
+      acc = add(acc, mul(r[i].z, r[i].z));
+      acc = add(acc, mul(r[i].w, r[i].w));
+    }
+    scalar_from = nvec * 4;
+  }
+  for (uint32_t e = scalar_from + threadIdx.x; e < len; e += kCNThreads) acc = add(acc, mul(p[e], p[e]));
+  const float r = block_sum(acc);
+  if (threadIdx.x == 0) part[b] = r;
+}
+
+// One CTA: thread t folds part[t], part[t + 256], ... in that order, then block_sum. The norm, and
+// the factor of utils.py:150-151 in float32 as the reference's scalar operators compute it:
+// _plus_scalar(1e-8), _rdiv_scalar(max_norm), min(concat(scale, 1)). A norm that is inf or nan
+// gives the factor 1, so the scaling pass leaves the arrays as they are.
+__global__ void __launch_bounds__(kCNThreads) clip_norm_fold_kernel(const float* part, uint32_t n_part,
+                                                                    float max_norm, float* total_norm,
+                                                                    float* scale) {
+  float acc = 0.f;
+  constexpr int kBatch = 8;  // loads in flight per thread; past the end they are +0.0f
+  for (uint32_t i0 = threadIdx.x; i0 < n_part; i0 += kBatch * kCNThreads) {
+    float v[kBatch];
+#pragma unroll
+    for (int j = 0; j < kBatch; ++j) {
+      const uint32_t i = i0 + j * kCNThreads;
+      v[j] = i < n_part ? part[i] : 0.f;
+    }
+#pragma unroll
+    for (int j = 0; j < kBatch; ++j) acc = add(acc, v[j]);
+  }
+  const float ss = block_sum(acc);
+  if (threadIdx.x == 0) {
+    const float norm = sqr(ss);
+    float s = dvd(max_norm, add(norm, 1e-8f));
+    s = s < 1.f ? s : 1.f;
+    *total_norm = norm;
+    *scale = isfinite(norm) ? s : 1.f;
+  }
+}
+
+// x = x * s in place. s == 1 is the identity on every finite value (and the factor the fold gives
+// for a non-finite norm), so the CTA returns before it reads anything.
+__global__ void __launch_bounds__(kCNThreads) clip_norm_scale_kernel(const ClipNormArrays A,
+                                                                     const float* scale_dev, float scale) {
+  const float s = scale_dev != nullptr ? *scale_dev : scale;
+  if (s == 1.f) return;
+  const uint32_t b = blockIdx.x;
+  const int k = cn_find(A, b);
+  const uint32_t e0 = (b - A.first_tile[k]) * kCNTileElems;
+  const uint32_t len = min(kCNTileElems, A.n[k] - e0);
+  float* p = A.p[k] + e0;
+  uint32_t scalar_from = 0;
+  if ((reinterpret_cast<uintptr_t>(A.p[k]) & 15) == 0) {
+    const uint32_t nvec = len / 4;
+    float4* v = reinterpret_cast<float4*>(p);
+    float4 r[kCNLoads];
+#pragma unroll
+    for (int i = 0; i < kCNLoads; ++i) {
+      const uint32_t j = threadIdx.x + i * kCNThreads;
+      if (j < nvec) r[i] = v[j];
+    }
+#pragma unroll
+    for (int i = 0; i < kCNLoads; ++i) {
+      const uint32_t j = threadIdx.x + i * kCNThreads;
+      if (j < nvec) v[j] = make_float4(mul(r[i].x, s), mul(r[i].y, s), mul(r[i].z, s), mul(r[i].w, s));
+    }
+    scalar_from = nvec * 4;
+  }
+  for (uint32_t e = scalar_from + threadIdx.x; e < len; e += kCNThreads) p[e] = mul(p[e], s);
+}
+
 template <class Op>
 void launch(const MTLaunch& L, cudaStream_t st) {
   mt_kernel<Op><<<L.n_chunks, kThreads, 0, st>>>(L.tensors, L.chunks, L.s, L.part0, L.part1);
@@ -504,6 +621,36 @@ void LaunchAllFinite(int dtype, AllFiniteArrays& A, float* out, cudaStream_t st)
     case kFloat64: all_finite_kernel<double><<<grid, kAFThreads, 0, st>>>(A, out); break;
     default: KV_FATAL << "all_finite: unsupported dtype " << DTypeName(dtype);
   }
+  KV_CUDA(cudaGetLastError());
+}
+
+uint32_t ClipNormTiles(ClipNormArrays& A) {
+  KV_CHECK(A.count >= 1 && A.count <= kCNMaxArrays);
+  uint32_t tiles = 0;  // <= 200 arrays x 2^20 tiles each
+  for (int i = 0; i < A.count; ++i) {
+    A.first_tile[i] = tiles;
+    tiles += static_cast<uint32_t>((static_cast<uint64_t>(A.n[i]) + kCNTileElems - 1) / kCNTileElems);
+  }
+  A.first_tile[A.count] = tiles;
+  return tiles;
+}
+
+void LaunchClipNormPartial(const ClipNormArrays& A, uint32_t tiles, float* part, cudaStream_t st) {
+  KV_CHECK(tiles >= 1 && tiles == A.first_tile[A.count]);
+  clip_norm_partial_kernel<<<tiles, kCNThreads, 0, st>>>(A, part);
+  KV_CUDA(cudaGetLastError());
+}
+
+void LaunchClipNormFold(const float* part, uint32_t n_part, float max_norm, float* total_norm,
+                        float* scale, cudaStream_t st) {
+  clip_norm_fold_kernel<<<1, kCNThreads, 0, st>>>(part, n_part, max_norm, total_norm, scale);
+  KV_CUDA(cudaGetLastError());
+}
+
+void LaunchClipNormScale(const ClipNormArrays& A, uint32_t tiles, const float* scale_dev, float scale,
+                         cudaStream_t st) {
+  KV_CHECK(tiles >= 1 && tiles == A.first_tile[A.count]);
+  clip_norm_scale_kernel<<<tiles, kCNThreads, 0, st>>>(A, scale_dev, scale);
   KV_CUDA(cudaGetLastError());
 }
 

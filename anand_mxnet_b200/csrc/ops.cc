@@ -36,6 +36,8 @@ const std::map<std::string, OpInfo>& Registry() {
           "_mp_adamw_update", "_multi_adamw_update", "_multi_mp_adamw_update", "lamb_update_phase1",
           "lamb_update_phase2", "mp_lamb_update_phase1", "mp_lamb_update_phase2",
           "_multi_lamb_update", "_multi_mp_lamb_update", "all_finite", "multi_all_finite",
+          // extensions: gradient clipping by global norm and the bulk unscale (multi_ops.cc)
+          "_b200kv_clip_global_norm", "_b200kv_multi_scale",
           // single-tensor operators of the callback route (update_ops.cc)
           "nag_mom_update", "mp_nag_mom_update", "signsgd_update", "signum_update", "rmsprop_update",
           "rmspropalex_update", "ftml_update", "ftrl_update", "_sparse_ftrl_update",

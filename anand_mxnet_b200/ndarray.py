@@ -661,5 +661,12 @@ class _Contrib(object):
     # row_sparse) or (dense, row_sparse, dense), history of shape (rows, 1); no wd parameter
     group_adagrad_update = staticmethod(_op('_contrib_group_adagrad_update'))
 
+    @staticmethod
+    def multi_scale(*arrays, scalar):
+        """x *= float32(scalar) in place for every array (float32, dense or row_sparse, one GPU) in
+        one launch per 200 arrays: the bulk form of amp.unscale's `g[:] *= scale`. The scalar is
+        parsed as `_mul_scalar` parses its own in the reference (std::stod, then rounded to float)."""
+        _invoke('_b200kv_multi_scale', list(arrays), num_arrays=len(arrays), scalar=scalar)
+
 
 contrib = _Contrib()

@@ -111,9 +111,12 @@ B200KV_DLL int MXNDArrayCallDLPackDeleter(DLManagedTensorHandle dlpack);        
  * (src/operator/optimizer_op.cc:322-710) and the elementwise helpers updaters use
  * (_copyto, _plus, _minus, _mul, _plus_scalar, _mul_scalar, _set_value, cast), the multi-tensor
  * operators (multi_sum_sq, multi_lars, preloaded_multi_*, AdamW, LAMB), the AMP overflow check
- * all_finite / multi_all_finite (src/operator/contrib/all_finite.cc) and the single-tensor
- * operators of the other optimizers (ops.cc lists them all). Any other name fails with
- * "operator not registered". */
+ * all_finite / multi_all_finite (src/operator/contrib/all_finite.cc), the single-tensor
+ * operators of the other optimizers (ops.cc lists them all), and two extensions the reference
+ * composes from NDArray arithmetic: _b200kv_clip_global_norm (inputs array_0 .. array_{n-1}, float32,
+ * scaled in place; parameters num_arrays, max_norm; output total_norm, a (1,) float32 array) and
+ * _b200kv_multi_scale (same inputs; parameters num_arrays, scalar; no output). Any other name fails
+ * with "operator not registered". */
 B200KV_DLL int NNGetOpHandle(const char* op_name, AtomicSymbolCreator* op_out);
 B200KV_DLL int MXImperativeInvokeEx(AtomicSymbolCreator creator, int num_inputs,
                                     NDArrayHandle* inputs, int* num_outputs,
