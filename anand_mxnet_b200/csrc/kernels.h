@@ -260,6 +260,22 @@ void LaunchClipNormFold(const float* part, uint32_t n_part, float max_norm, floa
 void LaunchClipNormScale(const ClipNormArrays& arrays, uint32_t tiles, const float* scale_dev, float scale,
                          cudaStream_t stream);
 
+// reset_arrays (contrib/reset_arrays.cc, ParameterDict.zero_grad): every byte of every array set to
+// 0x00, which is +0.0 in each floating dtype, so arrays of different dtypes share a launch. Listed
+// by value like AllFiniteArrays, tiled by bytes the same way; no byte outside [p, p + bytes) is
+// written. A call with more than kRAMaxArrays arrays goes group by group.
+constexpr int kRAMaxArrays = 200;
+constexpr int kRATileBytes = 16384;
+struct ResetArraysList {
+  void* p[kRAMaxArrays];                     // any alignment
+  uint64_t bytes[kRAMaxArrays];
+  uint32_t first_tile[kRAMaxArrays + 1];     // prefix of the tile counts (filled by the launcher)
+  int32_t count;
+};
+static_assert(sizeof(ResetArraysList) <= 32764, "kernel parameters are limited to 32764 bytes");
+// reset_arrays_kernel: one launch, none when every array is empty. Returns the number of launches.
+int LaunchResetArrays(ResetArraysList& arrays, cudaStream_t stream);
+
 // ---- single-tensor optimizer operators of the callback route (update_kernels.cu) ----
 // nag_mom_update, mp_nag_mom_update, signsgd_update, signum_update, rmsprop_update,
 // rmspropalex_update, ftml_update, ftrl_update (optimizer_op-inl.h:1061-1222, 1953-2158, 2344-2431)

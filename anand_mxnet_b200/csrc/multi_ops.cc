@@ -11,6 +11,7 @@
 //   lamb_update_phase1/2, mp_lamb_...     src/operator/optimizer_op.cc:926-1095
 //   _multi_lamb_update, _multi_mp_...     src/operator/contrib/multi_lamb.cc:174-251
 //   all_finite, multi_all_finite          src/operator/contrib/all_finite.cc:42-166
+//   reset_arrays                          src/operator/contrib/reset_arrays.cc:32-66
 // Extensions without a reference operator (the reference composes them from NDArray arithmetic):
 //   _b200kv_clip_global_norm              python/mxnet/gluon/utils.py:118-157
 //   _b200kv_multi_scale                   python/mxnet/contrib/amp/amp.py:340-346 (unscale)
@@ -409,6 +410,63 @@ bool MultiTensorOp(const std::string& n, const std::vector<NDArray>& in, std::ve
       Engine::Get()->CountLaunch("clip_norm_scale", 0);
     }
     op.Issue();
+    return true;
+  }
+  // ------------------------------------------------------------------------------- reset_arrays
+  if (n == "reset_arrays") {
+    for (const auto& kv : p) {  // ResetArraysParam::Init rejects unknown keys
+      KV_CHECK(kv.first == "num_arrays")
+          << "Cannot find argument '" << kv.first << "', Possible Arguments: num_arrays";
+    }
+    KV_CHECK(Find(p, "num_arrays") != nullptr) << "Required parameter num_arrays of " << n << " is missing";
+    const int num = GetI(p, "num_arrays", -1);
+    KV_CHECK(num >= 1) << n << ": num_arrays must be at least 1, got " << num;
+    KV_CHECK_EQ(static_cast<int>(in.size()), num) << n << ": expected num_arrays inputs";
+    KV_CHECK(outputs->empty()) << n << " zeroes its inputs in place and has no output";
+    KV_CHECK(in[0].on_gpu()) << n << " runs on GPU arrays only (no CPU fallback)";
+    const int dev = in[0].dev();
+    std::vector<ResetArraysList> groups;  // the dense arrays with bytes to write
+    for (int i = 0; i < num; ++i) {
+      const NDArray& a = in[i];
+      KV_CHECK(a.on_gpu() && a.dev() == dev)
+          << n << ": array_" << i << " is not on array_0's GPU; all operands must be on the same GPU "
+          << "(no CPU fallback)";
+      // MSHADOW_REAL_TYPE_SWITCH (mshadow/base.h:1130-1143), plus bfloat16 as all_finite serves it
+      switch (a.dtype()) {
+        case kFloat16: case kBfloat16: case kFloat32: case kFloat64: break;
+        case kUint8: KV_FATAL << "This operation only support floating point types not uint8";
+        case kInt8: KV_FATAL << "This operation only support floating point types not int8";
+        case kInt32: KV_FATAL << "This operation only support floating point types, not int32";
+        case kInt64: KV_FATAL << "This operation only support floating point types, not int64";
+        default: KV_FATAL << n << ": array_" << i << " has unsupported dtype " << DTypeName(a.dtype());
+      }
+      KV_CHECK(a.stype() == kDefaultStorage || a.stype() == kRowSparseStorage)
+          << n << ": array_" << i << " has csr storage; dense and row_sparse arrays are served";
+      if (a.stype() != kDefaultStorage || a.ByteSize() == 0) continue;
+      if (groups.empty() || groups.back().count == kRAMaxArrays) {
+        groups.emplace_back();
+        groups.back().count = 0;
+      }
+      ResetArraysList& g = groups.back();
+      g.p[g.count] = a.data();
+      g.bytes[g.count] = a.ByteSize();
+      ++g.count;
+    }
+    // every input is written (FMutateInputs): the zeroing follows pending readers and writers of
+    // each, and a pull anchor hands its value back to the store first
+    LaneOp op(dev);
+    for (const NDArray& a : in) op.Write(a);
+    Engine* eng = Engine::Get();
+    for (ResetArraysList& g : groups) {
+      if (LaunchResetArrays(g, op.stream()) > 0) eng->CountLaunch("reset_arrays", 0);
+    }
+    op.Issue();
+    // a row_sparse input keeps its storage and stores no rows, where the reference's storage
+    // fallback leaves it (dense temp, zeroed, cast back: imperative_utils.h:419-444). Work issued
+    // before this call read its rows already; the write declared above orders whatever follows.
+    for (const NDArray& a : in) {
+      if (a.stype() == kRowSparseStorage) a.SetNnr(0);
+    }
     return true;
   }
   // --------------------------------------------------------------------------------- multi_lars

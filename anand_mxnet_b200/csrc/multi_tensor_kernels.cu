@@ -2,7 +2,8 @@
 // (SURVEY 8f-f1): multi_sum_sq, multi_lars, _[mp_]adamw_update, _multi_[mp_]adamw_update,
 // [mp_]lamb_update_phase1/2, _multi_[mp_]lamb_update, the AMP overflow check
 // [multi_]all_finite (its own kernel and launch list, below), and gradient clipping by global
-// norm / the bulk unscale (_b200kv_clip_global_norm, _b200kv_multi_scale: three kernels, below).
+// norm / the bulk unscale (_b200kv_clip_global_norm, _b200kv_multi_scale: three kernels, below),
+// and reset_arrays (ParameterDict.zero_grad: one byte-wise kernel for every dtype, below).
 //
 // One launch covers every tensor of the call: a device table of MTTensor descriptors + a list of
 // <= 8192-element chunks (one 256-thread CTA each, 16-byte accesses, streaming loads/stores), the
@@ -390,6 +391,18 @@ template <> struct AfBits<double> {
   }
 };
 
+// The tiled launches below (all_finite, clip_norm_*, reset_arrays) give one CTA per tile of a list
+// of arrays; CTA b works on the last array whose first tile is <= b. Arrays without tiles share
+// their first tile with the next array and are never found.
+__device__ __forceinline__ int tile_owner(const uint32_t* first_tile, int count, uint32_t b) {
+  int lo = 0, hi = count - 1;
+  while (lo < hi) {
+    const int mid = (lo + hi + 1) >> 1;
+    if (first_tile[mid] <= b) lo = mid; else hi = mid - 1;
+  }
+  return lo;
+}
+
 // One CTA per tile; the CTA finds its array by a binary search over the first-tile prefix. A
 // 16-byte aligned array is read with kAFLoads independent 16-B loads per thread before any test
 // (plus a scalar tail in its last tile); any other base is read element by element. Default-cached
@@ -401,11 +414,7 @@ __global__ void __launch_bounds__(kAFThreads) all_finite_kernel(const AllFiniteA
   constexpr uint32_t kPerVec = 16 / sizeof(T);
   const uint32_t b = blockIdx.x;
   if (b >= A.first_tile[A.count]) return;  // the whole CTA: the launch of an all-empty list
-  int lo = 0, hi = A.count - 1;            // the last array whose first tile is <= b (not empty)
-  while (lo < hi) {
-    const int mid = (lo + hi + 1) >> 1;
-    if (A.first_tile[mid] <= b) lo = mid; else hi = mid - 1;
-  }
+  const int lo = tile_owner(A.first_tile, A.count, b);
   const uint64_t e0 = static_cast<uint64_t>(b - A.first_tile[lo]) * kTileElems;
   const uint32_t len = static_cast<uint32_t>(min(static_cast<uint64_t>(kTileElems), A.n[lo] - e0));
   const Raw* p = static_cast<const Raw*>(A.p[lo]) + e0;
@@ -441,21 +450,11 @@ constexpr int kCNLoads = kCNTileBytes / 16 / kCNThreads;
 constexpr uint32_t kCNTileElems = kCNTileBytes / sizeof(float);
 static_assert(kCNLoads * 16 * kCNThreads == kCNTileBytes, "a tile is whole loads of every thread");
 
-// the last array whose first tile is <= b (arrays without tiles are never found)
-__device__ __forceinline__ int cn_find(const ClipNormArrays& A, uint32_t b) {
-  int lo = 0, hi = A.count - 1;
-  while (lo < hi) {
-    const int mid = (lo + hi + 1) >> 1;
-    if (A.first_tile[mid] <= b) lo = mid; else hi = mid - 1;
-  }
-  return lo;
-}
-
 // part[blockIdx.x] = the tile's sum of x*x: per-thread sequential partial in element order, then
 // block_sum's fixed tree. Padding lanes add +0.0f, which leaves a sum of squares bitwise unchanged.
 __global__ void __launch_bounds__(kCNThreads) clip_norm_partial_kernel(const ClipNormArrays A, float* part) {
   const uint32_t b = blockIdx.x;
-  const int k = cn_find(A, b);
+  const int k = tile_owner(A.first_tile, A.count, b);
   const uint32_t e0 = (b - A.first_tile[k]) * kCNTileElems;
   const uint32_t len = min(kCNTileElems, A.n[k] - e0);
   const float* p = A.p[k] + e0;
@@ -520,7 +519,7 @@ __global__ void __launch_bounds__(kCNThreads) clip_norm_scale_kernel(const ClipN
   const float s = scale_dev != nullptr ? *scale_dev : scale;
   if (s == 1.f) return;
   const uint32_t b = blockIdx.x;
-  const int k = cn_find(A, b);
+  const int k = tile_owner(A.first_tile, A.count, b);
   const uint32_t e0 = (b - A.first_tile[k]) * kCNTileElems;
   const uint32_t len = min(kCNTileElems, A.n[k] - e0);
   float* p = A.p[k] + e0;
@@ -542,6 +541,44 @@ __global__ void __launch_bounds__(kCNThreads) clip_norm_scale_kernel(const ClipN
     scalar_from = nvec * 4;
   }
   for (uint32_t e = scalar_from + threadIdx.x; e < len; e += kCNThreads) p[e] = mul(p[e], s);
+}
+
+// ---------------------------------------------------------------------------------------------
+// reset_arrays (contrib/reset_arrays.cc; the reference runs one cudaMemsetAsync per array): zero
+// bytes whatever the dtype. One CTA per kRATileBytes tile of an array, counted from its base, found
+// as for all_finite_kernel. The 16-byte aligned body of a tile is written with kRAStores 16-B
+// stores per thread; the unaligned head and tail around it (< 16 bytes each, only when the base is
+// not 16-byte aligned, as for a[1:]) byte by byte. No byte outside [p, p + bytes) is written.
+// Default-cached stores: the next writer of a gradient is backward's accumulation (a streaming
+// hint has not been measured).
+constexpr int kRAThreads = 256;
+constexpr int kRAStores = kRATileBytes / 16 / kRAThreads;
+static_assert(kRAStores * 16 * kRAThreads == kRATileBytes, "a tile is whole stores of every thread");
+
+__global__ void __launch_bounds__(kRAThreads) reset_arrays_kernel(const ResetArraysList A) {
+  const uint32_t b = blockIdx.x;
+  const int k = tile_owner(A.first_tile, A.count, b);
+  const uint64_t off = static_cast<uint64_t>(b - A.first_tile[k]) * kRATileBytes;
+  const uint64_t len = min(static_cast<uint64_t>(kRATileBytes), A.bytes[k] - off);
+  unsigned char* lo = static_cast<unsigned char*>(A.p[k]) + off;
+  unsigned char* hi = lo + len;
+  uint4* v0 = reinterpret_cast<uint4*>((reinterpret_cast<uintptr_t>(lo) + 15) & ~static_cast<uintptr_t>(15));
+  uint4* v1 = reinterpret_cast<uint4*>(reinterpret_cast<uintptr_t>(hi) & ~static_cast<uintptr_t>(15));
+  if (reinterpret_cast<unsigned char*>(v0) >= reinterpret_cast<unsigned char*>(v1)) {
+    // no whole aligned 16 bytes in the tile (< 32 bytes): every byte alone
+    for (uint32_t e = threadIdx.x; e < len; e += kRAThreads) lo[e] = 0;
+    return;
+  }
+  const uint32_t nvec = static_cast<uint32_t>(v1 - v0);  // <= kRAStores * kRAThreads
+#pragma unroll
+  for (int i = 0; i < kRAStores; ++i) {
+    const uint32_t j = threadIdx.x + i * kRAThreads;
+    if (j < nvec) v0[j] = make_uint4(0u, 0u, 0u, 0u);
+  }
+  const uint32_t head = static_cast<uint32_t>(reinterpret_cast<unsigned char*>(v0) - lo);  // < 16
+  const uint32_t tail = static_cast<uint32_t>(hi - reinterpret_cast<unsigned char*>(v1));  // < 16
+  if (threadIdx.x < head) lo[threadIdx.x] = 0;
+  if (threadIdx.x >= 32 && threadIdx.x - 32 < tail) reinterpret_cast<unsigned char*>(v1)[threadIdx.x - 32] = 0;
 }
 
 template <class Op>
@@ -652,6 +689,21 @@ void LaunchClipNormScale(const ClipNormArrays& A, uint32_t tiles, const float* s
   KV_CHECK(tiles >= 1 && tiles == A.first_tile[A.count]);
   clip_norm_scale_kernel<<<tiles, kCNThreads, 0, st>>>(A, scale_dev, scale);
   KV_CUDA(cudaGetLastError());
+}
+
+int LaunchResetArrays(ResetArraysList& A, cudaStream_t st) {
+  KV_CHECK(A.count >= 1 && A.count <= kRAMaxArrays);
+  uint64_t tiles = 0;
+  for (int i = 0; i < A.count; ++i) {
+    A.first_tile[i] = static_cast<uint32_t>(tiles);
+    tiles += (A.bytes[i] + kRATileBytes - 1) / kRATileBytes;
+    KV_CHECK(tiles < (1ULL << 31)) << "reset_arrays: more than 2^31 tiles of " << kRATileBytes << " bytes";
+  }
+  A.first_tile[A.count] = static_cast<uint32_t>(tiles);
+  if (tiles == 0) return 0;
+  reset_arrays_kernel<<<static_cast<unsigned>(tiles), kRAThreads, 0, st>>>(A);
+  KV_CUDA(cudaGetLastError());
+  return 1;
 }
 
 }  // namespace b200kv

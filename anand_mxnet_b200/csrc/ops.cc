@@ -36,6 +36,7 @@ const std::map<std::string, OpInfo>& Registry() {
           "_mp_adamw_update", "_multi_adamw_update", "_multi_mp_adamw_update", "lamb_update_phase1",
           "lamb_update_phase2", "mp_lamb_update_phase1", "mp_lamb_update_phase2",
           "_multi_lamb_update", "_multi_mp_lamb_update", "all_finite", "multi_all_finite",
+          "reset_arrays", "_sparse_zeros_like",
           // extensions: gradient clipping by global norm and the bulk unscale (multi_ops.cc)
           "_b200kv_clip_global_norm", "_b200kv_multi_scale",
           // single-tensor operators of the callback route (update_ops.cc)
@@ -216,22 +217,30 @@ NDArray OutOrInput(std::vector<NDArray>* outputs, size_t i, const NDArray& like)
   return o;
 }
 
+// Dense operands only: the kernel walks Size() elements from data(), and a row_sparse array's
+// data() holds only its stored rows. Every check runs before anything is enqueued.
 void Elementwise(int op, const NDArray& a, const NDArray* b, float scalar, const NDArray& out) {
   KV_CHECK(out.on_gpu()) << "elementwise operators run on GPU arrays only";
+  KV_CHECK(out.stype() == kDefaultStorage)
+      << "elementwise operators take dense arrays only; out is not dense (default storage)";
   const int dev = out.dev();
-  LaneOp lop(dev);
   if (op != kEwFill) {
     KV_CHECK(a.on_gpu() && a.dev() == dev) << "all operands must be on the same GPU";
+    KV_CHECK(a.stype() == kDefaultStorage)
+        << "elementwise operators take dense arrays only; an input is not dense (default storage)";
     KV_CHECK_EQ(a.Size(), out.Size()) << "elementwise shape mismatch";
     KV_CHECK_EQ(a.dtype(), out.dtype()) << "elementwise dtype mismatch";
-    lop.Read(a);
   }
   if (b) {
     KV_CHECK(b->on_gpu() && b->dev() == dev) << "all operands must be on the same GPU";
+    KV_CHECK(b->stype() == kDefaultStorage)
+        << "elementwise operators take dense arrays only; an input is not dense (default storage)";
     KV_CHECK_EQ(b->Size(), out.Size()) << "elementwise shape mismatch";
     KV_CHECK_EQ(b->dtype(), out.dtype()) << "elementwise dtype mismatch";
-    lop.Read(*b);
   }
+  LaneOp lop(dev);
+  if (op != kEwFill) lop.Read(a);
+  if (b) lop.Read(*b);
   lop.Write(out);
   LaunchElementwise(op, out.dtype(), out.data(), op == kEwFill ? nullptr : a.data(),
                     b ? b->data() : nullptr, scalar, out.Size(), lop.stream());
@@ -398,10 +407,30 @@ void InvokeOp(const OpInfo* op, const std::vector<NDArray>& in, std::vector<NDAr
     Elementwise(kEwFill, NDArray(), nullptr, GetF(p, "src", 0.f), (*outputs)[0]);
     return;
   }
-  if (n == "zeros_like") {
+  if (n == "zeros_like" || n == "_sparse_zeros_like") {
     KV_CHECK_EQ(in.size(), 1u);
-    NDArray o = OutOrInput(outputs, 0, in[0]);
-    Elementwise(kEwFill, NDArray(), nullptr, 0.f, o);
+    const bool rsp_out = outputs->empty() ? in[0].stype() == kRowSparseStorage
+                                          : (*outputs)[0].stype() == kRowSparseStorage;
+    if (!rsp_out) {
+      NDArray o = OutOrInput(outputs, 0, in[0]);
+      Elementwise(kEwFill, NDArray(), nullptr, 0.f, o);
+      return;
+    }
+    // a row_sparse result stores no rows (FillZerosRspImpl, init_op.h:496-502): its storage is kept,
+    // nothing is launched. The write is declared first, so work issued before still sees the rows.
+    KV_CHECK(in[0].on_gpu()) << n << " runs on GPU arrays only (no CPU fallback)";
+    if (!outputs->empty()) {
+      const NDArray& o = (*outputs)[0];
+      KV_CHECK(o.on_gpu() && o.dev() == in[0].dev()) << "all operands must be on the same GPU";
+      KV_CHECK(o.shape() == in[0].shape()) << n << ": out shape mismatch";
+      KV_CHECK_EQ(o.dtype(), in[0].dtype()) << n << ": out dtype mismatch";
+    }
+    if (outputs->empty()) outputs->push_back(NDArray::RowSparse(in[0].shape(), in[0].ctx(), in[0].dtype()));
+    const NDArray& o = (*outputs)[0];
+    LaneOp op(o.dev());
+    op.Write(o);
+    op.Issue();
+    o.SetNnr(0);
     return;
   }
   if (n == "cast" || n == "Cast") {

@@ -550,6 +550,8 @@ ftrl_update = _op('ftrl_update')
 # (dense, row_sparse, dense) with wd = 0
 _Sparse.ftrl_update = staticmethod(_op('_sparse_ftrl_update'))
 _Sparse.adagrad_update = staticmethod(_op('_sparse_adagrad_update'))
+# mx.nd.sparse.zeros_like: the _sparse_zeros_like alias of zeros_like (init_op.cc:153-154)
+_Sparse.zeros_like = staticmethod(_op('_sparse_zeros_like'))
 cast = _op('cast')
 multi_sum_sq = _op('multi_sum_sq')
 multi_lars = _op('multi_lars')
@@ -558,6 +560,12 @@ multi_lars = _op('multi_lars')
 # inf or nan. multi_all_finite(*arrays, num_arrays=len(arrays), init_output=..., out=...)
 all_finite = _op('all_finite')
 multi_all_finite = _op('multi_all_finite')
+# ParameterDict.zero_grad's bulk reset: every input (float16 / bfloat16 / float32 / float64, one GPU)
+# zeroed in place, one launch per 200 dense arrays; row_sparse inputs end with no stored rows.
+# reset_arrays(*arrays, num_arrays=len(arrays)); no output
+reset_arrays = _op('reset_arrays')
+# zeros of data's shape and dtype; a row_sparse data or out gives a row_sparse array with no rows
+zeros_like = _op('zeros_like')
 preloaded_multi_sgd_update = _op('preloaded_multi_sgd_update')
 preloaded_multi_sgd_mom_update = _op('preloaded_multi_sgd_mom_update')
 preloaded_multi_mp_sgd_update = _op('preloaded_multi_mp_sgd_update')

@@ -111,7 +111,9 @@ B200KV_DLL int MXNDArrayCallDLPackDeleter(DLManagedTensorHandle dlpack);        
  * (src/operator/optimizer_op.cc:322-710) and the elementwise helpers updaters use
  * (_copyto, _plus, _minus, _mul, _plus_scalar, _mul_scalar, _set_value, cast), the multi-tensor
  * operators (multi_sum_sq, multi_lars, preloaded_multi_*, AdamW, LAMB), the AMP overflow check
- * all_finite / multi_all_finite (src/operator/contrib/all_finite.cc), the single-tensor
+ * all_finite / multi_all_finite (src/operator/contrib/all_finite.cc), zero_grad's reset_arrays
+ * (src/operator/contrib/reset_arrays.cc; inputs zeroed in place, no output) and zeros_like /
+ * _sparse_zeros_like on row_sparse arrays, the single-tensor
  * operators of the other optimizers (ops.cc lists them all), and two extensions the reference
  * composes from NDArray arithmetic: _b200kv_clip_global_norm (inputs array_0 .. array_{n-1}, float32,
  * scaled in place; parameters num_arrays, max_norm; output total_norm, a (1,) float32 array) and
