@@ -370,7 +370,8 @@ void KVStore::RunPrepared(Prepared& P) {
         L.beta2 = ScalarParam(opt_.beta2);
         L.eps = ScalarParam(opt_.eps);
       } else if (opt_kind == kOptTest) {
-        L.rescale = ScalarParam(opt_.rescale);
+        // Test.update's `grad * self.rescale_grad` is _mul_scalar: std::stod, then float32
+        L.rescale = StodParam(opt_.rescale);
       }
       P.hyper_version = opt_version_;
     }

@@ -1,8 +1,10 @@
 // misc_kernels.cu -- small elementwise kernels behind the imperative-op surface (custom updaters
 // written in the host language: `local += recv`, `weight[:] += grad * rescale`, casts, fills).
-// Not on the measured hot path; kept simple: 16-byte vector body + scalar tail, grid-stride.
+// Not on the measured hot path; kept simple: one element per thread, grid-stride.
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
+
+#include <type_traits>
 
 #include "common.h"
 #include "kernels.h"
@@ -10,53 +12,97 @@
 namespace b200kv {
 namespace {
 
-template <typename T> __device__ __forceinline__ float ToF(T x);
-template <> __device__ __forceinline__ float ToF<float>(float x) { return x; }
-template <> __device__ __forceinline__ float ToF<__half>(__half x) { return __half2float(x); }
-template <> __device__ __forceinline__ float ToF<__nv_bfloat16>(__nv_bfloat16 x) { return __bfloat162float(x); }
-template <> __device__ __forceinline__ float ToF<double>(double x) { return static_cast<float>(x); }
-template <> __device__ __forceinline__ float ToF<int32_t>(int32_t x) { return static_cast<float>(x); }
-template <> __device__ __forceinline__ float ToF<int64_t>(int64_t x) { return static_cast<float>(x); }
-template <> __device__ __forceinline__ float ToF<uint8_t>(uint8_t x) { return static_cast<float>(x); }
-template <> __device__ __forceinline__ float ToF<int8_t>(int8_t x) { return static_cast<float>(x); }
+// The 16-bit types compute in float and round once (half.h:45-66, MSHADOW_HALF_OPERATOR; bfloat16
+// is treated the same). Every other type computes in its own arithmetic, as mshadow_op's functors
+// do for float, double, int32 and int64.
+template <typename T> struct Is16 : std::false_type {};
+template <> struct Is16<__half> : std::true_type {};
+template <> struct Is16<__nv_bfloat16> : std::true_type {};
 
-template <typename T> __device__ __forceinline__ T FromF(float x);
-template <> __device__ __forceinline__ float FromF<float>(float x) { return x; }
-template <> __device__ __forceinline__ __half FromF<__half>(float x) { return __float2half_rn(x); }
-template <> __device__ __forceinline__ __nv_bfloat16 FromF<__nv_bfloat16>(float x) { return __float2bfloat16_rn(x); }
-template <> __device__ __forceinline__ double FromF<double>(float x) { return x; }
-template <> __device__ __forceinline__ int32_t FromF<int32_t>(float x) { return static_cast<int32_t>(x); }
-template <> __device__ __forceinline__ int64_t FromF<int64_t>(float x) { return static_cast<int64_t>(x); }
-template <> __device__ __forceinline__ uint8_t FromF<uint8_t>(float x) { return static_cast<uint8_t>(x); }
-template <> __device__ __forceinline__ int8_t FromF<int8_t>(float x) { return static_cast<int8_t>(x); }
+template <typename T> struct Calc { typedef T type; };
+template <> struct Calc<__half> { typedef float type; };
+template <> struct Calc<__nv_bfloat16> { typedef float type; };
 
-// mshadow evaluates 16-bit binary ops in float and rounds once (half.h:45-66); fp32 ops are plain
-// IEEE adds/muls (no contraction possible: one op per element).
+__device__ __forceinline__ float Widen(__half x) { return __half2float(x); }
+__device__ __forceinline__ float Widen(__nv_bfloat16 x) { return __bfloat162float(x); }
+template <typename T> __device__ __forceinline__ T Widen(T x) { return x; }
+
+// float -> T, rounding to nearest even: half_t's float constructor (half.h:322-330)
+template <typename T> __device__ __forceinline__ T FromFloat(float x) { return static_cast<T>(x); }
+template <> __device__ __forceinline__ __half FromFloat<__half>(float x) { return __float2half_rn(x); }
+template <> __device__ __forceinline__ __nv_bfloat16 FromFloat<__nv_bfloat16>(float x) {
+  return __float2bfloat16_rn(x);
+}
+
+template <typename T> __device__ __forceinline__ T Narrow(typename Calc<T>::type x) {
+  if constexpr (Is16<T>::value) return FromFloat<T>(x);
+  else return x;
+}
+
+// DType(alpha) for the double scalar of an operator; half_t(double) goes through float
+// (half.h:118, 322-330), and bfloat16 likewise. Integers truncate.
+template <typename T> __device__ __forceinline__ T FromDouble(double s) {
+  if constexpr (Is16<T>::value) return FromFloat<T>(__double2float_rn(s));
+  else return static_cast<T>(s);
+}
+
+__device__ __forceinline__ float Add(float a, float b) { return __fadd_rn(a, b); }
+__device__ __forceinline__ double Add(double a, double b) { return __dadd_rn(a, b); }
+template <typename I> __device__ __forceinline__ I Add(I a, I b) { return a + b; }
+__device__ __forceinline__ float Sub(float a, float b) { return __fsub_rn(a, b); }
+__device__ __forceinline__ double Sub(double a, double b) { return __dsub_rn(a, b); }
+template <typename I> __device__ __forceinline__ I Sub(I a, I b) { return a - b; }
+__device__ __forceinline__ float Mul(float a, float b) { return __fmul_rn(a, b); }
+__device__ __forceinline__ double Mul(double a, double b) { return __dmul_rn(a, b); }
+template <typename I> __device__ __forceinline__ I Mul(I a, I b) { return a * b; }
+// math::sqrt (math_functions-inl.h:43-55, 92): float in float, integers in double, then DType(...)
+__device__ __forceinline__ float Sqrt(float a) { return __fsqrt_rn(a); }
+__device__ __forceinline__ double Sqrt(double a) { return __dsqrt_rn(a); }
+template <typename I> __device__ __forceinline__ I Sqrt(I a) {
+  return static_cast<I>(__dsqrt_rn(static_cast<double>(a)));
+}
+
 template <typename T>
-__global__ void ew_kernel(int op, T* out, const T* a, const T* b, float scalar, size_t n) {
+__global__ void ew_kernel(int op, T* out, const T* a, const T* b, double scalar, size_t n) {
+  typedef typename Calc<T>::type C;
+  const T s = FromDouble<T>(scalar);
   for (size_t i = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; i < n;
        i += static_cast<size_t>(gridDim.x) * blockDim.x) {
-    float x = (op == kEwFill) ? 0.f : ToF<T>(a[i]);
-    float r;
-    switch (op) {
-      case kEwCopy: r = x; break;
-      case kEwAdd: r = __fadd_rn(x, ToF<T>(b[i])); break;
-      case kEwSub: r = __fsub_rn(x, ToF<T>(b[i])); break;
-      case kEwMul: r = __fmul_rn(x, ToF<T>(b[i])); break;
-      case kEwAddScalar: r = __fadd_rn(x, scalar); break;
-      case kEwMulScalar: r = __fmul_rn(x, scalar); break;
-      case kEwSqrt: r = __fsqrt_rn(x); break;
-      default: r = scalar; break;
+    if (op == kEwFill) {
+      out[i] = s;
+      continue;
     }
-    out[i] = FromF<T>(r);
+    if (op == kEwCopy) {
+      out[i] = a[i];
+      continue;
+    }
+    const C x = Widen(a[i]);
+    C r;
+    switch (op) {
+      case kEwAdd: r = Add(x, Widen(b[i])); break;
+      case kEwSub: r = Sub(x, Widen(b[i])); break;
+      case kEwMul: r = Mul(x, Widen(b[i])); break;
+      case kEwAddScalar: r = Add(x, Widen(s)); break;
+      case kEwMulScalar: r = Mul(x, Widen(s)); break;
+      default: r = Sqrt(x); break;  // kEwSqrt
+    }
+    out[i] = Narrow<T>(r);
   }
 }
 
+// tcast<TO>(in) (elemwise_unary_op.h:476): TO(x). A 16-bit side converts through float, as half_t
+// does (half.h:118-126, 322-330); every other pair converts directly.
 template <typename TO, typename TI>
 __global__ void cast_kernel(TO* out, const TI* in, size_t n) {
   for (size_t i = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; i < n;
        i += static_cast<size_t>(gridDim.x) * blockDim.x) {
-    out[i] = FromF<TO>(ToF<TI>(in[i]));
+    if constexpr (std::is_same<TO, TI>::value) {
+      out[i] = in[i];
+    } else if constexpr (Is16<TO>::value || Is16<TI>::value) {
+      out[i] = FromFloat<TO>(static_cast<float>(Widen(in[i])));
+    } else {
+      out[i] = static_cast<TO>(in[i]);
+    }
   }
 }
 
@@ -66,7 +112,7 @@ inline int GridFor(size_t n) {
 }
 
 template <typename T>
-void ew_launch(int op, void* out, const void* a, const void* b, float scalar, size_t n,
+void ew_launch(int op, void* out, const void* a, const void* b, double scalar, size_t n,
                cudaStream_t s) {
   ew_kernel<T><<<GridFor(n), 256, 0, s>>>(op, static_cast<T*>(out), static_cast<const T*>(a),
                                           static_cast<const T*>(b), scalar, n);
@@ -90,7 +136,12 @@ void cast_from(void* out, const void* in, int in_dtype, size_t n, cudaStream_t s
 
 }  // namespace
 
-void LaunchElementwise(int op, int dtype, void* out, const void* a, const void* b, float scalar,
+bool ElementwiseDTypeOk(int dtype) {
+  return dtype == kFloat32 || dtype == kFloat16 || dtype == kBfloat16 || dtype == kFloat64 ||
+         dtype == kInt32 || dtype == kInt64;
+}
+
+void LaunchElementwise(int op, int dtype, void* out, const void* a, const void* b, double scalar,
                        size_t n, cudaStream_t stream) {
   if (n == 0) return;
   switch (dtype) {

@@ -201,19 +201,6 @@ void CheckMP(const NDArray& w, bool mp, const std::string& op) {
   }
 }
 
-// the scalar of the reference's *_scalar operators: std::stod, then one rounding to the array's
-// dtype (elemwise_binary_scalar_op.h:364-365 and its `DType(alpha)`). Not GetF's dmlc::stof.
-float StodF(const Params& p, const char* key, const std::string& op) {
-  const std::string* v = Find(p, key);
-  KV_CHECK(v != nullptr) << "Required parameter " << key << " of " << op << " is missing";
-  try {
-    return static_cast<float>(std::stod(*v));
-  } catch (const std::exception&) {
-    KV_FATAL << op << ": cannot parse " << key << "='" << *v << "'";
-  }
-  return 0.f;
-}
-
 // per-GPU scratch of _b200kv_clip_global_norm: [0] the factor, [1 ...] the tile partials. Every
 // use is on the GPU's compute lane, so consecutive calls share it in stream order; it only grows.
 struct ClipScratch {

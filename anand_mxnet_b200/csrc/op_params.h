@@ -1,7 +1,9 @@
 // op_params.h -- the string attribute dict of an imperative operator call, parsed the way the
-// reference's dmlc::Parameter fields are (scalars: dmlc::stof; tuples: istream >> float).
+// reference's dmlc::Parameter fields are (scalars: dmlc::stof; tuples: istream >> float), and the
+// scalar of the *_scalar operators the way their attribute parser does (std::stod).
 #pragma once
 #include <cstdlib>
+#include <stdexcept>
 #include <string>
 #include <utility>
 #include <vector>
@@ -24,6 +26,25 @@ inline const std::string* Find(const Params& p, const std::string& k) {
 inline float GetF(const Params& p, const std::string& k, float dflt) {
   const std::string* v = Find(p, k);
   return v ? DmlcStof(*v) : dflt;
+}
+
+// the scalar of the reference's *_scalar operators: std::stod (elemwise_binary_scalar_op.h:347-354).
+// The kernel then rounds it once to the array's dtype, as BinaryScalarOp's DType(alpha) does.
+// Not GetF's dmlc::stof.
+inline double StodD(const Params& p, const char* key, const std::string& op) {
+  const std::string* v = Find(p, key);
+  KV_CHECK(v != nullptr) << "Required parameter " << key << " of " << op << " is missing";
+  try {
+    return std::stod(*v);
+  } catch (const std::exception&) {
+    KV_FATAL << op << ": cannot parse " << key << "='" << *v << "'";
+  }
+  return 0.0;
+}
+
+// the same for a float32 operand: std::stod, then one rounding to float
+inline float StodF(const Params& p, const char* key, const std::string& op) {
+  return static_cast<float>(StodD(p, key, op));
 }
 
 inline int GetI(const Params& p, const std::string& k, int dflt) {

@@ -29,7 +29,7 @@ const std::map<std::string, OpInfo>& Registry() {
          {"sgd_update", "sgd_mom_update", "mp_sgd_update", "mp_sgd_mom_update", "multi_sgd_update",
           "multi_sgd_mom_update", "multi_mp_sgd_update", "multi_mp_sgd_mom_update", "adam_update",
           "_copyto", "_plus", "elemwise_add", "_minus", "elemwise_sub", "_mul", "elemwise_mul",
-          "_plus_scalar", "_mul_scalar", "_set_value", "cast", "Cast", "zeros_like", "sqrt",
+          "_plus_scalar", "_mul_scalar", "_set_value", "_full", "cast", "Cast", "zeros_like", "sqrt",
           // multi-tensor optimizer operators (multi_ops.cc)
           "multi_sum_sq", "multi_lars", "preloaded_multi_sgd_update", "preloaded_multi_sgd_mom_update",
           "preloaded_multi_mp_sgd_update", "preloaded_multi_mp_sgd_mom_update", "_adamw_update",
@@ -219,10 +219,13 @@ NDArray OutOrInput(std::vector<NDArray>* outputs, size_t i, const NDArray& like)
 
 // Dense operands only: the kernel walks Size() elements from data(), and a row_sparse array's
 // data() holds only its stored rows. Every check runs before anything is enqueued.
-void Elementwise(int op, const NDArray& a, const NDArray* b, float scalar, const NDArray& out) {
+void Elementwise(int op, const NDArray& a, const NDArray* b, double scalar, const NDArray& out) {
   KV_CHECK(out.on_gpu()) << "elementwise operators run on GPU arrays only";
   KV_CHECK(out.stype() == kDefaultStorage)
       << "elementwise operators take dense arrays only; out is not dense (default storage)";
+  KV_CHECK(ElementwiseDTypeOk(out.dtype()))
+      << "elementwise operators take float16, bfloat16, float32, float64, int32 and int64 arrays; got "
+      << DTypeName(out.dtype());
   const int dev = out.dev();
   if (op != kEwFill) {
     KV_CHECK(a.on_gpu() && a.dev() == dev) << "all operands must be on the same GPU";
@@ -393,18 +396,29 @@ void InvokeOp(const OpInfo* op, const std::vector<NDArray>& in, std::vector<NDAr
     KV_CHECK_EQ(in.size(), 1u);
     NDArray o = OutOrInput(outputs, 0, in[0]);
     Elementwise(n == "_plus_scalar" ? kEwAddScalar : kEwMulScalar, in[0], nullptr,
-                GetF(p, "scalar", 0.f), o);
+                StodD(p, "scalar", n), o);
     return;
   }
   if (n == "sqrt") {
     KV_CHECK_EQ(in.size(), 1u);
     NDArray o = OutOrInput(outputs, 0, in[0]);
-    Elementwise(kEwSqrt, in[0], nullptr, 0.f, o);
+    Elementwise(kEwSqrt, in[0], nullptr, 0.0, o);
     return;
   }
   if (n == "_set_value") {
     KV_CHECK(outputs->size() == 1) << "_set_value needs an out array";
     Elementwise(kEwFill, NDArray(), nullptr, GetF(p, "src", 0.f), (*outputs)[0]);
+    return;
+  }
+  if (n == "_full") {
+    // `a[:] = v` (ndarray.py:504): InitOpWithScalarParam's double `value`, parsed by dmlc::stod, then
+    // Fill's static_cast<DType> (init_op.h:241-257, 416-421). Only into an existing out here.
+    KV_CHECK(outputs->size() == 1) << "_full needs an out array";
+    const std::string* v = Find(p, "value");
+    KV_CHECK(v != nullptr) << "Required parameter value of _full is missing";
+    double val = DmlcStod(*v);
+    if (val == 0) val = 0.0;  // Fill's val == 0 branch writes zero bytes: -0.0 stores +0.0
+    Elementwise(kEwFill, NDArray(), nullptr, val, (*outputs)[0]);
     return;
   }
   if (n == "zeros_like" || n == "_sparse_zeros_like") {
@@ -413,7 +427,7 @@ void InvokeOp(const OpInfo* op, const std::vector<NDArray>& in, std::vector<NDAr
                                           : (*outputs)[0].stype() == kRowSparseStorage;
     if (!rsp_out) {
       NDArray o = OutOrInput(outputs, 0, in[0]);
-      Elementwise(kEwFill, NDArray(), nullptr, 0.f, o);
+      Elementwise(kEwFill, NDArray(), nullptr, 0.0, o);
       return;
     }
     // a row_sparse result stores no rows (FillZerosRspImpl, init_op.h:496-502): its storage is kept,
@@ -453,6 +467,8 @@ void InvokeOp(const OpInfo* op, const std::vector<NDArray>& in, std::vector<NDAr
       o = (*outputs)[0];
     }
     KV_CHECK(in[0].on_gpu() && o.on_gpu() && in[0].dev() == o.dev()) << "cast runs on one GPU";
+    KV_CHECK_EQ(o.dtype(), dtype) << "cast: out dtype differs from dtype=" << *dt;
+    KV_CHECK_EQ(o.Size(), in[0].Size()) << "cast: out shape mismatch";
     LaneOp op(o.dev());
     op.Read(in[0]).Write(o);
     LaunchCast(o.data(), o.dtype(), in[0].data(), in[0].dtype(), o.Size(), op.stream());

@@ -7,6 +7,7 @@
 #include <cstdint>
 #include <cstdlib>
 #include <limits>
+#include <type_traits>
 
 #include "common.h"
 
@@ -62,11 +63,18 @@ std::string PyFloatRepr(double v) {
   return out;
 }
 
-// Restatement of ParseFloat<float, true> (3rdparty/dmlc-core/include/dmlc/strtonum.h:99-254).
-float DmlcStof(const std::string& s) {
-  constexpr unsigned kMaxExponent = 38U;
-  constexpr float kMaxSigForMaxExp = 3.402823466f;
-  constexpr float kMaxSigForNegMaxExp = 1.175494351f;
+namespace {
+
+// Restatement of ParseFloat<FloatType, true> (3rdparty/dmlc-core/include/dmlc/strtonum.h:99-254):
+// every step is taken in FloatType, as there.
+template <typename FloatType>
+FloatType ParseDmlc(const std::string& s) {
+  constexpr bool kDouble = std::is_same<FloatType, double>::value;
+  constexpr unsigned kMaxExponent = kDouble ? 308U : 38U;
+  constexpr FloatType kMaxSigForMaxExp =
+      static_cast<FloatType>(kDouble ? 1.79769313486231570 : 3.402823466);
+  constexpr FloatType kMaxSigForNegMaxExp =
+      static_cast<FloatType>(kDouble ? 2.22507385850720139 : 1.175494351);
   constexpr int kStrtofMaxDigits = 19;
   const char* p = s.c_str();
   const char* begin = p;
@@ -78,9 +86,10 @@ float DmlcStof(const std::string& s) {
   } else if (*p == '+') {
     ++p;
   }
-  auto finish = [&](float value, const char* end) -> float {
+  auto finish = [&](FloatType value, const char* end) -> FloatType {
     if (end == begin || *end != '\0') {
-      KV_FATAL << "Invalid Parameter format: expect float but value='" << s << "'";
+      KV_FATAL << "Invalid Parameter format: expect " << (kDouble ? "double" : "float")
+               << " but value='" << s << "'";
     }
     return value;
   };
@@ -88,13 +97,13 @@ float DmlcStof(const std::string& s) {
     int i = 0;
     while (i < 8 && static_cast<char>((*p) | 32) == "infinity"[i]) { ++i; ++p; }
     if (i == 3 || i == 8) {
-      return finish(positive ? std::numeric_limits<float>::infinity()
-                             : -std::numeric_limits<float>::infinity(), p);
+      return finish(positive ? std::numeric_limits<FloatType>::infinity()
+                             : -std::numeric_limits<FloatType>::infinity(), p);
     }
     p -= i;
     i = 0;
     while (i < 3 && static_cast<char>((*p) | 32) == "nan"[i]) { ++i; ++p; }
-    if (i == 3) return finish(std::numeric_limits<float>::quiet_NaN(), p);
+    if (i == 3) return finish(std::numeric_limits<FloatType>::quiet_NaN(), p);
     p -= i;
   }
   const char* num_start = p;
@@ -102,7 +111,7 @@ float DmlcStof(const std::string& s) {
   for (; std::isdigit(static_cast<unsigned char>(*p)); ++p) {
     predec = predec * 10ULL + static_cast<uint64_t>(*p - '0');
   }
-  float value = static_cast<float>(predec);
+  FloatType value = static_cast<FloatType>(predec);
   if (*p == '.') {
     uint64_t pow10 = 1, val2 = 0;
     int digit_cnt = 0;
@@ -115,13 +124,16 @@ float DmlcStof(const std::string& s) {
       ++p;
       ++digit_cnt;
     }
-    value += static_cast<float>(static_cast<double>(val2) / static_cast<double>(pow10));
+    value += static_cast<FloatType>(static_cast<double>(val2) / static_cast<double>(pow10));
   }
-  if (p == num_start) KV_FATAL << "Invalid Parameter format: expect float but value='" << s << "'";
+  if (p == num_start) {
+    KV_FATAL << "Invalid Parameter format: expect " << (kDouble ? "double" : "float")
+             << " but value='" << s << "'";
+  }
   if (*p == 'e' || *p == 'E') {
     ++p;
     bool frac = false;
-    float scale = 1.0f;
+    FloatType scale = static_cast<FloatType>(1.0f);
     unsigned expon = 0;
     if (*p == '-') {
       frac = true;
@@ -137,12 +149,18 @@ float DmlcStof(const std::string& s) {
                                   (frac && value < kMaxSigForNegMaxExp))) {
       KV_FATAL << "Out of range value '" << s << "'";
     }
-    while (expon >= 8U) { scale *= 1E8f; expon -= 8U; }
-    while (expon > 0U) { scale *= 10.0f; expon -= 1U; }
+    while (expon >= 8U) { scale *= static_cast<FloatType>(1E8f); expon -= 8U; }
+    while (expon > 0U) { scale *= static_cast<FloatType>(10.0f); expon -= 1U; }
     value = frac ? (value / scale) : (value * scale);
   }
   if (*p == 'f' || *p == 'F') ++p;
   return finish(positive ? value : -value, p);
 }
+
+}  // namespace
+
+float DmlcStof(const std::string& s) { return ParseDmlc<float>(s); }
+
+double DmlcStod(const std::string& s) { return ParseDmlc<double>(s); }
 
 }  // namespace b200kv

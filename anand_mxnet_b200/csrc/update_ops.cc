@@ -54,89 +54,6 @@ const Spec kSpecs[] = {
     {"_contrib_group_adagrad_update", kUpdGroupAdaGrad, 3, "update_op(_contrib_group_adagrad_update)", 12},
 };
 
-// Restatement of dmlc::stod == ParseFloat<double, true> (3rdparty/dmlc-core/include/dmlc/
-// strtonum.h:99-254, 497-510), the parser of double fields (FieldEntry<double>, parameter.h:1106-1125)
-// such as FTML's epsilon. Like stof it is not correctly rounded: float(int part) + double(frac
-// digits) / double(10^k), then scaled by powers of ten.
-double DmlcStod(const std::string& s) {
-  constexpr unsigned kMaxExponent = 308U;
-  constexpr double kMaxSigForMaxExp = 1.79769313486231570;
-  constexpr double kMaxSigForNegMaxExp = 2.22507385850720139;
-  constexpr int kStrtofMaxDigits = 19;
-  const char* p = s.c_str();
-  while (std::isspace(static_cast<unsigned char>(*p))) ++p;
-  bool positive = true;
-  if (*p == '-') {
-    positive = false;
-    ++p;
-  } else if (*p == '+') {
-    ++p;
-  }
-  auto finish = [&](double value, const char* end) -> double {
-    KV_CHECK(end != s.c_str() && *end == '\0')
-        << "Invalid Parameter format: expect double but value='" << s << "'";
-    return value;
-  };
-  {
-    int i = 0;
-    while (i < 8 && static_cast<char>((*p) | 32) == "infinity"[i]) { ++i; ++p; }
-    if (i == 3 || i == 8) {
-      return finish(positive ? std::numeric_limits<double>::infinity()
-                             : -std::numeric_limits<double>::infinity(), p);
-    }
-    p -= i;
-    i = 0;
-    while (i < 3 && static_cast<char>((*p) | 32) == "nan"[i]) { ++i; ++p; }
-    if (i == 3) return finish(std::numeric_limits<double>::quiet_NaN(), p);
-    p -= i;
-  }
-  const char* num_start = p;
-  uint64_t predec = 0;
-  for (; std::isdigit(static_cast<unsigned char>(*p)); ++p) {
-    predec = predec * 10ULL + static_cast<uint64_t>(*p - '0');
-  }
-  double value = static_cast<double>(predec);
-  if (*p == '.') {
-    uint64_t pow10 = 1, val2 = 0;
-    int digit_cnt = 0;
-    ++p;
-    while (std::isdigit(static_cast<unsigned char>(*p))) {
-      if (digit_cnt < kStrtofMaxDigits) {
-        val2 = val2 * 10ULL + static_cast<uint64_t>(*p - '0');
-        pow10 *= 10ULL;
-      }
-      ++p;
-      ++digit_cnt;
-    }
-    value += static_cast<double>(val2) / static_cast<double>(pow10);
-  }
-  KV_CHECK(p != num_start) << "Invalid Parameter format: expect double but value='" << s << "'";
-  if (*p == 'e' || *p == 'E') {
-    ++p;
-    bool frac = false;
-    double scale = 1.0;
-    unsigned expon = 0;
-    if (*p == '-') {
-      frac = true;
-      ++p;
-    } else if (*p == '+') {
-      ++p;
-    }
-    for (; std::isdigit(static_cast<unsigned char>(*p)); ++p) {
-      expon = expon * 10U + static_cast<unsigned>(*p - '0');
-    }
-    KV_CHECK(expon <= kMaxExponent) << "Out of range value '" << s << "'";
-    KV_CHECK(!(expon == kMaxExponent && ((!frac && value > kMaxSigForMaxExp) ||
-                                         (frac && value < kMaxSigForNegMaxExp))))
-        << "Out of range value '" << s << "'";
-    while (expon >= 8U) { scale *= static_cast<double>(1E8f); expon -= 8U; }
-    while (expon > 0U) { scale *= static_cast<double>(10.0f); expon -= 1U; }
-    value = frac ? (value / scale) : (value * scale);
-  }
-  if (*p == 'f' || *p == 'F') ++p;
-  return finish(positive ? value : -value, p);
-}
-
 float Required(const Params& p, const char* key, const std::string& op) {
   KV_CHECK(Find(p, key) != nullptr) << "Required parameter " << key << " of " << op << " is missing";
   return GetF(p, key, 0.f);

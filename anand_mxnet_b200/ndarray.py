@@ -267,7 +267,8 @@ class NDArray(object):
                 value.copyto(self)
         elif isinstance(value, (int, float, np.generic)):
             if self.context.device_type == 'gpu':
-                _invoke('_set_value', [], out=self, src=float(value))
+                # the reference's _full (ndarray.py:504): value=float(value), cast to the dtype
+                _invoke('_full', [], out=self, value=float(value))
             else:
                 self._sync_copyfrom(np.full(self.shape, value))
         else:

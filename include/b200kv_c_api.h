@@ -109,7 +109,7 @@ B200KV_DLL int MXNDArrayCallDLPackDeleter(DLManagedTensorHandle dlpack);        
  * Registered ops: sgd_update, sgd_mom_update, mp_sgd_update, mp_sgd_mom_update, multi_sgd_update,
  * multi_sgd_mom_update, multi_mp_sgd_update, multi_mp_sgd_mom_update, adam_update
  * (src/operator/optimizer_op.cc:322-710) and the elementwise helpers updaters use
- * (_copyto, _plus, _minus, _mul, _plus_scalar, _mul_scalar, _set_value, cast), the multi-tensor
+ * (_copyto, _plus, _minus, _mul, _plus_scalar, _mul_scalar, _set_value, _full, cast), the multi-tensor
  * operators (multi_sum_sq, multi_lars, preloaded_multi_*, AdamW, LAMB), the AMP overflow check
  * all_finite / multi_all_finite (src/operator/contrib/all_finite.cc), zero_grad's reset_arrays
  * (src/operator/contrib/reset_arrays.cc; inputs zeroed in place, no output) and zeros_like /

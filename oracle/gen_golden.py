@@ -124,6 +124,10 @@ def updater_cases():
     cases['lars_list'] = dict(lplan(3), opt=('LARS', dict(momentum=0.9, wd=1e-4, eta=0.02, eps=1e-6, rescale_grad=1 / 32)),
                               sched=('FactorScheduler', dict(step=2, factor=0.5, base_lr=0.4)), lr_at=[0.4, 0.4, 0.2])
     cases['lamb_list'] = dict(lplan(3), opt=('LAMB', dict(learning_rate=2e-3, wd=0.01, rescale_grad=0.25)))
+    # a rescale_grad whose dmlc::stof and std::stod-then-float parses differ: Test's `grad * rescale_grad`
+    # is _mul_scalar, which takes std::stod (appended last so that no earlier case's draws move)
+    cases['test_rescale_stod'] = dict(plan(3), opt=('Test', dict(rescale_grad=1.2345e-05)),
+                                      model=dict(kind='test', rescale_grad=1.2345e-05))
     return cases
 
 

@@ -921,8 +921,8 @@ class LocalKVStoreModel(object):
                                sp(lr_t), sp(p['beta1']), sp(p['beta2']), sp(p['eps']), sp(wd),
                                sp(p['rescale']), sp(clip) if clip else None)
         elif p['kind'] == 'test':
-            # grad * rescale_grad -> _mul_scalar(scalar=str(rescale_grad))
-            self.o.test_update(w.reshape(-1), merged.reshape(-1), sp(p['rescale']))
+            # grad * rescale_grad -> _mul_scalar(scalar=str(rescale_grad)): std::stod, then float32
+            self.o.test_update(w.reshape(-1), merged.reshape(-1), f32(p['rescale']))
         else:
             raise ValueError(p['kind'])
 

@@ -37,7 +37,9 @@ REF_PY = "/root/reference/python/mxnet"
 
 def available():
     r = K.ref()
-    return os.path.isfile(os.path.join(REF_PY, "optimizer", "optimizer.py")) and r is not None and r.has_ops()
+    import golden_ndarray_ops as GN
+    return os.path.isfile(os.path.join(REF_PY, "optimizer", "optimizer.py")) and r is not None and r.has_ops() \
+        and GN.ref() is not None
 
 
 class Context(object):
@@ -86,10 +88,12 @@ class NDArray(object):
         self.a[key] = value.a if isinstance(value, NDArray) else value
 
     def __mul__(self, scalar):
-        # NDArray * python scalar -> _mul_scalar(scalar=str(scalar)): the scalar goes through dmlc::stof
+        # NDArray * python scalar -> _mul_scalar(scalar=str(float(scalar))): the operator's own
+        # registered parser (std::stod), DType(alpha) and mshadow_op::mul, from _ref/libmxref_ndarith.so
+        import golden_ndarray_ops as GN
         LOG.append(('_mul_scalar', {'scalar': str(scalar)}))
-        s = np.float32(K.ref().dmlc_stof(repr(float(scalar))))
-        return NDArray((self.a * s).astype(self.a.dtype), self.context)
+        out = GN.ref().binary_scalar('mul', self.a, repr(float(scalar)), np.dtype(self.a.dtype).name)
+        return NDArray(out.reshape(self.a.shape), self.context)
 
     def __iadd__(self, other):
         self.a += other.a

@@ -240,7 +240,7 @@ def test_fused_test_optimizer(mx):
                shapes=[(4, 4), (100, 100), (2000, 2000)], rng=rng)
 
 
-@pytest.mark.parametrize("optname", ['sgd', 'adam'])
+@pytest.mark.parametrize("optname", ['sgd', 'adam', 'test'])
 def test_callback_route_equals_fused_route(mx, optname, monkeypatch):
     """The reference's route (store -> Python Updater -> optimizer operators) and the fused route
     must agree bit-for-bit, including update counts and Adam's bias-corrected lr."""
@@ -257,8 +257,10 @@ def test_callback_route_equals_fused_route(mx, optname, monkeypatch):
         from compat import mxnet_optimizer as mxopt
         if optname == 'sgd':
             opt = mxopt.SGD(learning_rate=0.05, momentum=0.9, wd=1e-3, rescale_grad=0.5)
-        else:
+        elif optname == 'adam':
             opt = mxopt.Adam(learning_rate=2e-3, wd=0.02, rescale_grad=0.25)
+        else:   # dmlc::stof and std::stod-then-float parse this rescale_grad differently
+            opt = mxopt.Test(rescale_grad=1.2345e-05)
         kv.set_optimizer(opt)
         assert (kv._fused is not None) == (fused == '1')
         outs = [mx.nd.empty(s, mx.gpu(0)) for s in shapes]

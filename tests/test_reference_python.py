@@ -153,6 +153,8 @@ CONFIGS = {
     'lamb_bounds_nobias': lambda m, s: m.LAMB(learning_rate=1e-3, lower_bound=0.01, upper_bound=2.0,
                                               bias_correction=False, clip_gradient=0.4),
     'test': lambda m, s: m.Test(rescale_grad=2.0),
+    # dmlc::stof and std::stod-then-float parse this rescale_grad to different floats
+    'test_rescale_stod': lambda m, s: m.Test(rescale_grad=1.2345e-05),
 }
 
 
@@ -209,7 +211,7 @@ def _compare(cfg, mode, dtype=np.float32, steps=5, monkeypatch=None, agg=None, m
 
 @live
 @pytest.mark.parametrize("mode", ['single', 'list'])
-@pytest.mark.parametrize("cfg", sorted(c for c in CONFIGS if c != 'test'))
+@pytest.mark.parametrize("cfg", sorted(c for c in CONFIGS if not c.startswith('test')))
 def test_compat_mirror_vs_reference(cfg, mode):
     _compare(cfg, mode)
 
@@ -217,6 +219,12 @@ def test_compat_mirror_vs_reference(cfg, mode):
 @live
 def test_compat_mirror_test_optimizer():
     _compare('test', 'single')
+
+
+@live
+def test_compat_mirror_test_optimizer_stod_rescale():
+    """grad * rescale_grad is _mul_scalar: the reference's registered parser, not dmlc::stof"""
+    _compare('test_rescale_stod', 'single')
 
 
 @live

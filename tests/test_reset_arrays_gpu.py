@@ -445,7 +445,7 @@ def test_refusals_leave_every_operand_unchanged(mx):
     d = f32.view
     like = mx.nd.array(np.ones((10, 4), np.float32), mx.gpu(0))
     refused = [
-        lambda: a.__setitem__(slice(None), 1.0),                                   # _set_value
+        lambda: a.__setitem__(slice(None), 1.0),                                   # _full
         lambda: like + a, lambda: a + like, lambda: a + 2.0, lambda: a * 3.0,      # _plus, _plus_scalar, _mul_scalar
         lambda: mx.nd._invoke('_plus', [like, like], out=a),
         lambda: mx.nd._invoke('_mul_scalar', [like], out=a, scalar=2.0),

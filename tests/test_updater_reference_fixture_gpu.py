@@ -4,7 +4,7 @@ written by oracle/gen_golden.py through oracle/ref_python.py: python/mxnet/optim
 Updater / SGD / Adam / Test + lr_scheduler.FactorScheduler, src/operator/optimizer_op.cc
 FCompute<cpu>). No oracle in between; weights bit for bit after every case's last step -- update
 counts, multipliers, the scheduler call, Adam's bias correction and the python-repr -> dmlc::stof
-scalar route all have to agree for that."""
+scalar route (std::stod for Test's `grad * rescale_grad`, a _mul_scalar) all have to agree for that."""
 import numpy as np
 import pytest
 
@@ -47,9 +47,9 @@ def test_store_trajectory_golden(mx, golden, name, fused, monkeypatch):
                 return case['lr_at'][min(max(num_update, 1), len(case['lr_at'])) - 1]
         kw['lr_scheduler'] = Sched()
     if cls == 'Test':
-        if fused == '0':
-            pytest.skip("the 'test' optimizer of tests/nightly/test_kvstore.py is exercised on the fused route")
-        opt = mx.optimizer.Test(**kw)
+        # fused: the package's record; callback: the reference's Test class, whose update() runs
+        # `weight += grad * rescale_grad` through _mul_scalar and _plus
+        opt = mx.optimizer.Test(**kw) if fused == '1' else mxopt.Test(**kw)
     else:
         opt = getattr(mxopt, cls)(**kw)
     if case.get('lr_mult'):
