@@ -58,6 +58,10 @@ std::shared_ptr<MTPlan> GetPlan(int dev, int op, std::vector<MTTensor>* tensors,
   for (auto& t : *tensors) {
     for (void* p : t.p) sig = Mix(sig, reinterpret_cast<uint64_t>(p));
     sig = Mix(sig, (static_cast<uint64_t>(t.size) << 32) | t.aux);
+    // vec_ok depends on the operands' dtypes as well as their addresses (a float16 array at an
+    // 8-byte aligned address is vectorised, a float32 one there is not): a table cached for one
+    // dtype must not serve another at the same addresses
+    sig = Mix(sig, t.vec_ok);
   }
   auto& cache = Plans();
   auto it = cache.find(sig);
@@ -70,8 +74,11 @@ std::shared_ptr<MTPlan> GetPlan(int dev, int op, std::vector<MTTensor>* tensors,
   for (size_t i = 0; i < tensors->size(); ++i) {
     MTTensor& t = (*tensors)[i];
     t.first_chunk = static_cast<uint32_t>(chunks.size());
-    for (uint32_t off = 0; off < t.size; off += kMTChunk) {
-      chunks.push_back(MTChunk{static_cast<uint32_t>(i), off, std::min<uint32_t>(kMTChunk, t.size - off), 0});
+    // 64-bit offset: for a size in (2^32 - kMTChunk, 2^32) a uint32 offset would wrap past the
+    // last chunk and the loop would never end. Every chunk's own offset still fits in uint32.
+    for (uint64_t off = 0; off < t.size; off += kMTChunk) {
+      chunks.push_back(MTChunk{static_cast<uint32_t>(i), static_cast<uint32_t>(off),
+                               static_cast<uint32_t>(std::min<uint64_t>(kMTChunk, t.size - off)), 0});
     }
   }
   plan->n_tensors = static_cast<int>(tensors->size());
@@ -484,6 +491,7 @@ bool MultiTensorOp(const std::string& n, const std::vector<NDArray>& in, std::ve
     const bool mp = n.find("_mp_") != std::string::npos;
     const int stride = mp ? 5 : 4;
     const int num = multi ? GetI(p, "num_weights", 1) : 1;
+    KV_CHECK(num >= 1) << n << ": num_weights must be at least 1, got " << num;
     KV_CHECK_EQ(static_cast<int>(in.size()), num * stride + 1)
         << n << ": expected " << (multi ? "num_weights*" : "") << stride << " + 1 inputs";
     const NDArray& rescale = in[num * stride];
@@ -638,6 +646,7 @@ bool MultiTensorOp(const std::string& n, const std::vector<NDArray>& in, std::ve
     const bool mp = n.find("_mp_") != std::string::npos;
     const int stride = mp ? 5 : 4;
     const int num = GetI(p, "num_tensors", 1);
+    KV_CHECK(num >= 1) << n << ": num_tensors must be at least 1, got " << num;
     KV_CHECK(num <= 45) << "Invalid number of tensors, the maximum value is 45, and got " << num;
     KV_CHECK_EQ(static_cast<int>(in.size()), num * stride) << n << ": expected num_tensors*" << stride << " inputs";
     std::vector<float> lrs = GetTuple(p, "learning_rates"), wds = GetTuple(p, "wds");

@@ -326,7 +326,7 @@ __global__ void __launch_bounds__(kThreads) mt_finalize_kernel(const MTTensor* t
                                                                const float* part0, const float* part1,
                                                                float* out0, float* out1) {
   const MTTensor t = tensors[blockIdx.x];
-  const uint32_t n = (t.size + kMTChunk - 1) / kMTChunk;
+  const uint32_t n = static_cast<uint32_t>((static_cast<uint64_t>(t.size) + kMTChunk - 1) / kMTChunk);
   float a0 = 0.f, a1 = 0.f;
   for (uint32_t i = threadIdx.x; i < n; i += kThreads) {
     a0 = __fadd_rn(a0, part0[t.first_chunk + i]);
