@@ -3,8 +3,10 @@
 // scalar of the *_scalar operators the way their attribute parser does (std::stod).
 #pragma once
 #include <cstdlib>
+#include <initializer_list>
 #include <stdexcept>
 #include <string>
+#include <type_traits>
 #include <utility>
 #include <vector>
 
@@ -28,22 +30,46 @@ inline float GetF(const Params& p, const std::string& k, float dflt) {
   return v ? DmlcStof(*v) : dflt;
 }
 
+// a parameter without a default value, refused when absent (dmlc::Parameter::Init): float fields
+// parsed as GetF does, int fields as GetI, double fields with dmlc::stod, or the string itself
+template <typename T = float>
+T Required(const Params& p, const char* key, const char* op) {
+  const std::string* v = Find(p, key);
+  KV_CHECK(v != nullptr) << "Required parameter " << key << " of " << op << " is missing";
+  if constexpr (std::is_same<T, std::string>::value) return *v;
+  else if constexpr (std::is_same<T, int>::value) return std::atoi(v->c_str());
+  else if constexpr (std::is_same<T, double>::value) return DmlcStod(*v);
+  else return DmlcStof(*v);
+}
+
+// dmlc::Parameter::Init refuses a key its parameter struct does not declare, listing those it does
+inline void RejectUnknownKeys(const Params& p, std::initializer_list<const char*> allowed) {
+  for (const auto& kv : p) {
+    bool known = false;
+    std::string list;
+    for (const char* k : allowed) {
+      known = known || kv.first == k;
+      list += (list.empty() ? "" : ", ") + std::string(k);
+    }
+    KV_CHECK(known) << "Cannot find argument '" << kv.first << "', Possible Arguments: " << list;
+  }
+}
+
 // the scalar of the reference's *_scalar operators: std::stod (elemwise_binary_scalar_op.h:347-354).
 // The kernel then rounds it once to the array's dtype, as BinaryScalarOp's DType(alpha) does.
 // Not GetF's dmlc::stof.
-inline double StodD(const Params& p, const char* key, const std::string& op) {
-  const std::string* v = Find(p, key);
-  KV_CHECK(v != nullptr) << "Required parameter " << key << " of " << op << " is missing";
+inline double StodD(const Params& p, const char* key, const char* op) {
+  const std::string v = Required<std::string>(p, key, op);
   try {
-    return std::stod(*v);
+    return std::stod(v);
   } catch (const std::exception&) {
-    KV_FATAL << op << ": cannot parse " << key << "='" << *v << "'";
+    KV_FATAL << op << ": cannot parse " << key << "='" << v << "'";
   }
   return 0.0;
 }
 
 // the same for a float32 operand: std::stod, then one rounding to float
-inline float StodF(const Params& p, const char* key, const std::string& op) {
+inline float StodF(const Params& p, const char* key, const char* op) {
   return static_cast<float>(StodD(p, key, op));
 }
 

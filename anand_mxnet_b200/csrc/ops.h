@@ -2,29 +2,74 @@
 // operators (src/operator/optimizer_op.cc:195-710) plus the few elementwise helpers that updaters
 // written in the host language rely on. All run on the arrays' GPU through the dense fused kernel.
 #pragma once
+#include <cstdint>
+#include <map>
+#include <memory>
 #include <string>
 #include <utility>
 #include <vector>
 
 #include "ndarray.h"
+#include "op_params.h"
 
 namespace b200kv {
 
+struct OpInfo;
+// outputs: caller-provided (in place) or empty -> allocated and appended
+typedef void (*OpFn)(const OpInfo& op, const std::vector<NDArray>& inputs, std::vector<NDArray>* outputs,
+                     const Params& params);
+
+// One operator: its name, its handler, and what the handler varies on (a kernel op code, kOp* flag
+// bits, or an index into the family's own table). Handlers use `name` in error messages only.
 struct OpInfo {
-  std::string name;
+  const char* name;
+  OpFn run;
+  int variant;
 };
+
+// variant bits of the operators that come in plain, mom, mp, multi and preloaded forms
+enum OpFlags { kOpMom = 1, kOpMp = 2, kOpMulti = 4, kOpPreloaded = 8 };
+
+// each family's operators: ops.cc, multi_ops.cc, update_ops.cc
+extern const std::vector<OpInfo> kCoreOps, kMultiTensorOps, kUpdateOps;
 
 // nullptr when the operator is not registered
 const OpInfo* FindOp(const std::string& name);
 
-// outputs: caller-provided (in place) or empty -> allocated and appended
+// runs op->run; a malformed rescale_grad or clip_gradient is refused first, whichever the operator
 void InvokeOp(const OpInfo* op, const std::vector<NDArray>& inputs, std::vector<NDArray>* outputs,
-              const std::vector<std::pair<std::string, std::string>>& params);
+              const Params& params);
 
-// multi_ops.cc: the multi-tensor optimizer operators (multi_sum_sq, multi_lars, adamw, lamb);
-// returns false when `name` is not one of them
-bool MultiTensorOp(const std::string& name, const std::vector<NDArray>& inputs,
-                   std::vector<NDArray>* outputs,
-                   const std::vector<std::pair<std::string, std::string>>& params);
+// outputs[i], or a new array appended to outputs when the caller passed fewer
+NDArray OutOr(std::vector<NDArray>* outputs, size_t i, const std::vector<int64_t>& shape, Context ctx,
+              int dtype);
+// the front-end passes out=weight; a distinct out receives the weight first (then updated in place)
+NDArray InPlace(const std::vector<NDArray>& in, size_t widx, std::vector<NDArray>* outputs, size_t oidx);
+
+// Device copies of the descriptor tables an operator call builds from its operands, kept per
+// operand list so that a repeated call uploads nothing. The key holds everything the tables were
+// built from (addresses, sizes, flags) and a hit compares it in full. Past 512 entries the whole
+// cache is dropped. Each caller builds its own tables and keeps its own cache.
+class TableCache {
+ public:
+  struct Tables {
+    explicit Tables(int dev) : dev(dev) {}
+    int dev;
+    int n_chunks = 0;
+    void* d[3] = {};
+    size_t bytes[3] = {};
+    // buffer i: `size` bytes on dev, the first `host_bytes` of them copied from `host`
+    void Upload(int i, size_t size, const void* host, size_t host_bytes, cudaStream_t st);
+    ~Tables();
+  };
+  // the tables of `key`, or nullptr
+  const Tables* Find(const std::vector<uint64_t>& key) const;
+  // stores tables the caller has filled in full: an entry is never seen half built, and tables
+  // whose filling threw are freed by their owner instead
+  const Tables* Insert(std::vector<uint64_t> key, std::unique_ptr<Tables> tables);
+
+ private:
+  std::map<std::vector<uint64_t>, std::unique_ptr<Tables>> map_;
+};
 
 }  // namespace b200kv

@@ -54,11 +54,6 @@ const Spec kSpecs[] = {
     {"_contrib_group_adagrad_update", kUpdGroupAdaGrad, 3, "update_op(_contrib_group_adagrad_update)", 12},
 };
 
-float Required(const Params& p, const char* key, const std::string& op) {
-  KV_CHECK(Find(p, key) != nullptr) << "Required parameter " << key << " of " << op << " is missing";
-  return GetF(p, key, 0.f);
-}
-
 // dmlc::Parameter set_range(lo, hi) (parameter.h:752-762)
 float InRange(float v, const char* key, float lo, float hi) {
   KV_CHECK(!(v < lo || v > hi)) << "value " << v << " for Parameter " << key << " exceed bound [" << lo
@@ -79,7 +74,7 @@ const char* StypeName(int stype) { return stype == kRowSparseStorage ? "row_spar
 //   _contrib_group_adagrad_update       the same two forms; history has one value per row
 void RspUpdateOp(const Spec& spec, const std::vector<NDArray>& in, std::vector<NDArray>* outputs,
                  const Params& p) {
-  const std::string n = spec.name;
+  const char* n = spec.name;
   const int op = spec.op;
   const NDArray& w = in[0];
   const NDArray& g = in[1];
@@ -98,12 +93,7 @@ void RspUpdateOp(const Spec& spec, const std::vector<NDArray>& in, std::vector<N
         << n << ": the row_sparse form needs row_sparse weight, grad, z and n (a dense weight with a "
         << "row_sparse gradient is not supported)";
   } else if (op == kUpdGroupAdaGrad) {  // GroupAdagradParam (contrib/optimizer_op-inl.h:46-65)
-    for (const auto& kv : p) {  // dmlc::Parameter::Init rejects unknown keys (wd among them)
-      KV_CHECK(kv.first == "lr" || kv.first == "rescale_grad" || kv.first == "clip_gradient" ||
-               kv.first == "epsilon")
-          << "Cannot find argument '" << kv.first << "', Possible Arguments: lr, rescale_grad, "
-          << "clip_gradient, epsilon";
-    }
+    RejectUnknownKeys(p, {"lr", "rescale_grad", "clip_gradient", "epsilon"});  // wd among the unknown
     L.eps = GetF(p, "epsilon", 1.0e-5f);
     const int hst = in[2].stype();
     // all-dense operands dispatch to an FCompute the reference does not register
@@ -152,8 +142,7 @@ void RspUpdateOp(const Spec& spec, const std::vector<NDArray>& in, std::vector<N
   // kWriteInplace is expected (optimizer_op-inl.h:2235, 2572)
   KV_CHECK(outputs->size() == 1 && (*outputs)[0].SameStorage(w) && (*outputs)[0].stype() == wst &&
            (*outputs)[0].data() == w.data())
-      << n << ": out must be the weight itself (kWriteInplace is expected for sparse " << spec.name
-      << ")";
+      << n << ": out must be the weight itself (kWriteInplace is expected for sparse " << n << ")";
 
   Engine* eng = Engine::Get();
   LaneOp lop(w.dev());
@@ -192,17 +181,14 @@ void RspUpdateOp(const Spec& spec, const std::vector<NDArray>& in, std::vector<N
   lop.Issue();
 }
 
-}  // namespace
-
-bool UpdateOp(const std::string& n, const std::vector<NDArray>& in, std::vector<NDArray>* outputs,
+// every operator of kSpecs (variant: its index there): the row_sparse forms in RspUpdateOp, the
+// dense ones here
+void UpdateOp(const OpInfo& info, const std::vector<NDArray>& in, std::vector<NDArray>* outputs,
               const Params& p) {
-  const Spec* spec = nullptr;
-  for (const Spec& s : kSpecs) {
-    if (n == s.name) spec = &s;
-  }
-  if (spec == nullptr) return false;
-  const int op = spec->op;
-  KV_CHECK_EQ(static_cast<int>(in.size()), spec->nin) << n << " expects " << spec->nin << " inputs";
+  const Spec& spec = kSpecs[info.variant];
+  const char* n = spec.name;
+  const int op = spec.op;
+  KV_CHECK_EQ(static_cast<int>(in.size()), spec.nin) << n << " expects " << spec.nin << " inputs";
   const NDArray& w = in[0];
   const NDArray& g = in[1];
   if (op == kUpdFtrl) {  // FtrlUpdateEx (optimizer_op-inl.h:2303-2306)
@@ -213,8 +199,8 @@ bool UpdateOp(const std::string& n, const std::vector<NDArray>& in, std::vector<
     }
   }
   if (op == kUpdAdaGrad || op == kUpdGroupAdaGrad || w.stype() == kRowSparseStorage) {
-    RspUpdateOp(*spec, in, outputs, p);
-    return true;
+    RspUpdateOp(spec, in, outputs, p);
+    return;
   }
   for (const NDArray& a : in) {
     KV_CHECK(a.stype() == kDefaultStorage)
@@ -236,17 +222,11 @@ bool UpdateOp(const std::string& n, const std::vector<NDArray>& in, std::vector<
   }
   KV_CHECK_EQ(g.dtype(), dtype) << n << ": weight / grad dtype mismatch";
   KV_CHECK_EQ(g.Size(), w.Size()) << n << ": weight / grad shape mismatch";
-  for (int i = 2; i < spec->nin; ++i) {
+  for (int i = 2; i < spec.nin; ++i) {
     KV_CHECK_EQ(in[i].dtype(), kFloat32) << n << ": optimizer states must be float32";
     KV_CHECK_EQ(in[i].Size(), w.Size()) << n << ": state shape mismatch";
   }
-  NDArray out;
-  if (outputs->empty()) {
-    out = NDArray(w.shape(), w.ctx(), dtype);
-    outputs->push_back(out);
-  } else {
-    out = (*outputs)[0];
-  }
+  NDArray out = OutOr(outputs, 0, w.shape(), w.ctx(), dtype);
   KV_CHECK(out.on_gpu() && out.dev() == dev) << n << ": out must be on the weight's GPU";
   KV_CHECK(out.stype() == kDefaultStorage) << n << ": out must be a dense array";
   KV_CHECK_EQ(out.dtype(), dtype) << n << ": out dtype mismatch";
@@ -282,8 +262,7 @@ bool UpdateOp(const std::string& n, const std::vector<NDArray>& in, std::vector<
       L.beta2 = InRange(GetF(p, "beta2", 0.999f), "beta2", 0.f, 1.f);
       const std::string* e = Find(p, "epsilon");
       L.eps = static_cast<float>(e ? DmlcStod(*e) : static_cast<double>(1e-8f));
-      KV_CHECK(Find(p, "t") != nullptr) << "Required parameter t of " << n << " is missing";
-      const int t = GetI(p, "t", 0);
+      const int t = Required<int>(p, "t", n);
       L.clip = GetF(p, "clip_grad", -1.0f);
       // power::Map(beta, DType(t)) is ::powf of the host C library (math_functions-inl.h:58-61,126):
       // evaluated here once per call rather than with the device's powf
@@ -299,7 +278,7 @@ bool UpdateOp(const std::string& n, const std::vector<NDArray>& in, std::vector<
   L.w = w.data();
   L.g = g.data();
   L.out = out.data();
-  for (int i = 2; i < spec->nin; ++i) L.s[i - 2] = static_cast<float*>(in[i].data());
+  for (int i = 2; i < spec.nin; ++i) L.s[i - 2] = static_cast<float*>(in[i].data());
   L.n = w.Size();
   L.out_is_w = out_is_w;
 
@@ -307,11 +286,18 @@ bool UpdateOp(const std::string& n, const std::vector<NDArray>& in, std::vector<
   lop.Read(g);
   if (!out_is_w) lop.Read(w);
   lop.Write(out);
-  for (int i = 2; i < spec->nin; ++i) lop.Write(in[i]);
+  for (int i = 2; i < spec.nin; ++i) lop.Write(in[i]);
   LaunchUpdateOp(L, lop.stream());
-  Engine::Get()->CountLaunch(spec->launch_name, static_cast<uint64_t>(spec->bytes_per_elem) * L.n);
+  Engine::Get()->CountLaunch(spec.launch_name, static_cast<uint64_t>(spec.bytes_per_elem) * L.n);
   lop.Issue();
-  return true;
 }
+
+}  // namespace
+
+const std::vector<OpInfo> kUpdateOps = [] {
+  std::vector<OpInfo> rows;
+  for (const Spec& s : kSpecs) rows.push_back({s.name, UpdateOp, static_cast<int>(&s - kSpecs)});
+  return rows;
+}();
 
 }  // namespace b200kv

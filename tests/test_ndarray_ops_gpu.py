@@ -77,6 +77,7 @@ def fill(mx, n, dt, seed):
 # --------------------------------------------------------------------------------- array ops
 IOP = {'plus': '__iadd__', 'minus': '__isub__', 'mul': '__imul__'}
 NAME = {'plus': '_plus', 'minus': '_minus', 'mul': '_mul'}
+ALIAS = {'plus': 'elemwise_add', 'minus': 'elemwise_sub', 'mul': 'elemwise_mul'}
 
 
 @pytest.mark.parametrize("case", G.array_cases(), ids=lambda c: c[0])
@@ -99,9 +100,11 @@ def test_array_operator(mx, fixture, case):
     got = down({'plus': A + B, 'minus': A - B, 'mul': A * B}[op], dt)
     check(got, want, dt, name)
     check_fixture(fixture, name, got, dt)
-    O, _ = fill(mx, n, dt, 2)
-    mx.nd._invoke(NAME[op], [A, B], out=O)
-    check(down(O, dt), want, dt, name + ' out=')
+    for opname in (NAME[op], ALIAS[op]):
+        O, _ = fill(mx, n, dt, 2)
+        mx.nd._invoke(opname, [A, B], out=O)
+        check(down(O, dt), want, dt, '%s %s out=' % (name, opname))
+        check_fixture(fixture, name, down(O, dt), dt)
     check(down(A, dt), a, dt, name + ' input kept')
     R = getattr(A, IOP[op])(B)                                  # a op= b
     assert R is A
@@ -172,6 +175,11 @@ def test_assignment(mx, fixture, dt):
         got = down(A, dt)
         check(got, G.full(v, n, dt), dt, '%s (value %r)' % (name, v))
         check_fixture(fixture, name, got, dt)
+    if dt == 'float32':
+        # _set_value: a fill from its float src, with a value float32 holds exactly
+        A, _ = fill(mx, 4099, dt, 3)
+        mx.nd._invoke('_set_value', [], out=A, src=0.375)
+        check(down(A, dt), G.full(0.375, 4099, dt), dt, '_set_value')
 
 
 # ---------------------------------------------------------------------------------------- casts
@@ -183,9 +191,10 @@ def test_cast(mx, fixture, src, dst):
         x = G.inputs('cast', case)[0]
         want = G.restate('cast', case)
         X = up(mx, x, src)
-        got = down(X.astype(dst), dst)
-        check(got, want, dst, case[0])
-        check_fixture(fixture, case[0], got, dst)
+        for result in (X.astype(dst), mx.nd._invoke('Cast', [X], dtype=dst)):
+            got = down(result, dst)
+            check(got, want, dst, case[0])
+            check_fixture(fixture, case[0], got, dst)
         if n <= 4099:
             O, _ = fill(mx, n, dst, 4)
             mx.nd.cast(X, dtype=dst, out=O)
