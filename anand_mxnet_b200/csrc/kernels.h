@@ -94,10 +94,15 @@ void LaunchDenseFused(const DenseLaunch& p, cudaStream_t stream);
 // ---- small elementwise helpers for the imperative-op surface (updaters written in Python) ----
 // float16, bfloat16, float32, float64, int32 and int64. `scalar` is the operator's double; the kernel
 // converts it once to the array's dtype, as the reference's DType(alpha) / static_cast<DType>(value).
-enum EwOp : int { kEwCopy = 0, kEwAdd, kEwSub, kEwMul, kEwAddScalar, kEwMulScalar, kEwFill, kEwSqrt };
+// kEwClip takes its float bounds a_min, a_max as `scalar`, `scalar2` and compares them with each
+// element as the reference's clip kernel does. kEwDiv and kEwDivScalar divide floating types only.
+enum EwOp : int {
+  kEwCopy = 0, kEwAdd, kEwSub, kEwMul, kEwAddScalar, kEwMulScalar, kEwFill, kEwSqrt,
+  kEwDiv, kEwMax, kEwDivScalar, kEwAbs, kEwClip
+};
 bool ElementwiseDTypeOk(int dtype);
 void LaunchElementwise(int op, int dtype, void* out, const void* a, const void* b, double scalar,
-                       size_t n, cudaStream_t stream);
+                       size_t n, cudaStream_t stream, double scalar2 = 0.0);
 void LaunchCast(void* out, int out_dtype, const void* in, int in_dtype, size_t n, cudaStream_t stream);
 
 // ---- row_sparse (rowsparse_kernels.cu) ----

@@ -61,9 +61,32 @@ __device__ __forceinline__ double Sqrt(double a) { return __dsqrt_rn(a); }
 template <typename I> __device__ __forceinline__ I Sqrt(I a) {
   return static_cast<I>(__dsqrt_rn(static_cast<double>(a)));
 }
+// mshadow_op::div (mshadow_op.h:352): a / b. Integer arrays never reach it: the operators refuse them.
+__device__ __forceinline__ float Div(float a, float b) { return __fdiv_rn(a, b); }
+__device__ __forceinline__ double Div(double a, double b) { return __ddiv_rn(a, b); }
+template <typename I> __device__ __forceinline__ I Div(I a, I b) { return a / b; }
+// mshadow_op::maximum (mshadow_op.h:1083-1092): a NaN `a` is returned, else a > b ? a : b, so a NaN
+// `b` and equal values (-0 against +0) give b. `a != a` is IsNan for floats and false for integers.
+template <typename C> __device__ __forceinline__ C Max(C a, C b) { return a != a ? a : (a > b ? a : b); }
+// mshadow_op::abs over math::fabs (mshadow_op.h:545, math_functions-inl.h:43-55): fabsf for float,
+// fabs for double, integers through double and back
+__device__ __forceinline__ float Abs(float a) { return fabsf(a); }
+__device__ __forceinline__ double Abs(double a) { return fabs(a); }
+template <typename I> __device__ __forceinline__ I Abs(I a) {
+  return static_cast<I>(fabs(static_cast<double>(a)));
+}
+// the clip kernel (matrix_op-inl.h:1604-1617): each element against the float bounds in C++'s
+// arithmetic, so an integer converts to float and a double compares with the widened bound; a
+// bound taken is converted to the dtype (the 16-bit types round it from float). NaN falls through.
+template <typename C> __device__ __forceinline__ C Clip(C x, float lo, float hi) {
+  if (x > hi) return static_cast<C>(hi);
+  if (x < lo) return static_cast<C>(lo);
+  return x;
+}
 
 template <typename T>
-__global__ void ew_kernel(int op, T* out, const T* a, const T* b, double scalar, size_t n) {
+__global__ void ew_kernel(int op, T* out, const T* a, const T* b, double scalar, double scalar2,
+                          size_t n) {
   typedef typename Calc<T>::type C;
   const T s = FromDouble<T>(scalar);
   for (size_t i = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; i < n;
@@ -84,6 +107,11 @@ __global__ void ew_kernel(int op, T* out, const T* a, const T* b, double scalar,
       case kEwMul: r = Mul(x, Widen(b[i])); break;
       case kEwAddScalar: r = Add(x, Widen(s)); break;
       case kEwMulScalar: r = Mul(x, Widen(s)); break;
+      case kEwDiv: r = Div(x, Widen(b[i])); break;
+      case kEwMax: r = Max(x, Widen(b[i])); break;
+      case kEwDivScalar: r = Div(x, Widen(s)); break;
+      case kEwAbs: r = Abs(x); break;
+      case kEwClip: r = Clip(x, static_cast<float>(scalar), static_cast<float>(scalar2)); break;
       default: r = Sqrt(x); break;  // kEwSqrt
     }
     out[i] = Narrow<T>(r);
@@ -112,10 +140,10 @@ inline int GridFor(size_t n) {
 }
 
 template <typename T>
-void ew_launch(int op, void* out, const void* a, const void* b, double scalar, size_t n,
-               cudaStream_t s) {
+void ew_launch(int op, void* out, const void* a, const void* b, double scalar, double scalar2,
+               size_t n, cudaStream_t s) {
   ew_kernel<T><<<GridFor(n), 256, 0, s>>>(op, static_cast<T*>(out), static_cast<const T*>(a),
-                                          static_cast<const T*>(b), scalar, n);
+                                          static_cast<const T*>(b), scalar, scalar2, n);
 }
 
 template <typename TO>
@@ -142,15 +170,15 @@ bool ElementwiseDTypeOk(int dtype) {
 }
 
 void LaunchElementwise(int op, int dtype, void* out, const void* a, const void* b, double scalar,
-                       size_t n, cudaStream_t stream) {
+                       size_t n, cudaStream_t stream, double scalar2) {
   if (n == 0) return;
   switch (dtype) {
-    case kFloat32: ew_launch<float>(op, out, a, b, scalar, n, stream); break;
-    case kFloat16: ew_launch<__half>(op, out, a, b, scalar, n, stream); break;
-    case kBfloat16: ew_launch<__nv_bfloat16>(op, out, a, b, scalar, n, stream); break;
-    case kFloat64: ew_launch<double>(op, out, a, b, scalar, n, stream); break;
-    case kInt32: ew_launch<int32_t>(op, out, a, b, scalar, n, stream); break;
-    case kInt64: ew_launch<int64_t>(op, out, a, b, scalar, n, stream); break;
+    case kFloat32: ew_launch<float>(op, out, a, b, scalar, scalar2, n, stream); break;
+    case kFloat16: ew_launch<__half>(op, out, a, b, scalar, scalar2, n, stream); break;
+    case kBfloat16: ew_launch<__nv_bfloat16>(op, out, a, b, scalar, scalar2, n, stream); break;
+    case kFloat64: ew_launch<double>(op, out, a, b, scalar, scalar2, n, stream); break;
+    case kInt32: ew_launch<int32_t>(op, out, a, b, scalar, scalar2, n, stream); break;
+    case kInt64: ew_launch<int64_t>(op, out, a, b, scalar, scalar2, n, stream); break;
     default: KV_FATAL << "elementwise op: unsupported dtype " << DTypeName(dtype);
   }
   KV_CUDA(cudaGetLastError());

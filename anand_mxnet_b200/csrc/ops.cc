@@ -51,7 +51,7 @@ NDArray InPlace(const std::vector<NDArray>& in, size_t widx, std::vector<NDArray
 const OpInfo* FindOp(const std::string& name) {
   static const auto* table = [] {
     auto* m = new std::unordered_map<std::string, const OpInfo*>();
-    for (const std::vector<OpInfo>* family : {&kCoreOps, &kMultiTensorOps, &kUpdateOps}) {
+    for (const std::vector<OpInfo>* family : {&kCoreOps, &kMultiTensorOps, &kUpdateOps, &kArithOps}) {
       for (const OpInfo& op : *family) {
         KV_CHECK(m->emplace(op.name, &op).second) << "operator " << op.name << " is declared twice";
       }
@@ -60,6 +60,41 @@ const OpInfo* FindOp(const std::string& name) {
   }();
   auto it = table->find(name);
   return it == table->end() ? nullptr : it->second;
+}
+
+// Dense operands only: the kernel walks Size() elements from data(), and a row_sparse array's
+// data() holds only its stored rows. Every check runs before anything is enqueued.
+void Elementwise(int op, const NDArray& a, const NDArray* b, double scalar, const NDArray& out,
+                 double scalar2) {
+  KV_CHECK(out.on_gpu()) << "elementwise operators run on GPU arrays only";
+  KV_CHECK(out.stype() == kDefaultStorage)
+      << "elementwise operators take dense arrays only; out is not dense (default storage)";
+  KV_CHECK(ElementwiseDTypeOk(out.dtype()))
+      << "elementwise operators take float16, bfloat16, float32, float64, int32 and int64 arrays; got "
+      << DTypeName(out.dtype());
+  const int dev = out.dev();
+  if (op != kEwFill) {
+    KV_CHECK(a.on_gpu() && a.dev() == dev) << "all operands must be on the same GPU";
+    KV_CHECK(a.stype() == kDefaultStorage)
+        << "elementwise operators take dense arrays only; an input is not dense (default storage)";
+    KV_CHECK_EQ(a.Size(), out.Size()) << "elementwise shape mismatch";
+    KV_CHECK_EQ(a.dtype(), out.dtype()) << "elementwise dtype mismatch";
+  }
+  if (b) {
+    KV_CHECK(b->on_gpu() && b->dev() == dev) << "all operands must be on the same GPU";
+    KV_CHECK(b->stype() == kDefaultStorage)
+        << "elementwise operators take dense arrays only; an input is not dense (default storage)";
+    KV_CHECK_EQ(b->Size(), out.Size()) << "elementwise shape mismatch";
+    KV_CHECK_EQ(b->dtype(), out.dtype()) << "elementwise dtype mismatch";
+  }
+  LaneOp lop(dev);
+  if (op != kEwFill) lop.Read(a);
+  if (b) lop.Read(*b);
+  lop.Write(out);
+  LaunchElementwise(op, out.dtype(), out.data(), op == kEwFill ? nullptr : a.data(),
+                    b ? b->data() : nullptr, scalar, out.Size(), lop.stream(), scalar2);
+  Engine::Get()->CountLaunch("elementwise", 0);
+  lop.Issue();
 }
 
 namespace {
@@ -185,40 +220,6 @@ void RunRspUpdate(int opt, const NDArray& w, const NDArray& g, const NDArray& s1
   LaunchRspUpdate(L, op.stream());
   Engine::Get()->CountLaunch("rsp_update", 0);
   op.Issue();
-}
-
-// Dense operands only: the kernel walks Size() elements from data(), and a row_sparse array's
-// data() holds only its stored rows. Every check runs before anything is enqueued.
-void Elementwise(int op, const NDArray& a, const NDArray* b, double scalar, const NDArray& out) {
-  KV_CHECK(out.on_gpu()) << "elementwise operators run on GPU arrays only";
-  KV_CHECK(out.stype() == kDefaultStorage)
-      << "elementwise operators take dense arrays only; out is not dense (default storage)";
-  KV_CHECK(ElementwiseDTypeOk(out.dtype()))
-      << "elementwise operators take float16, bfloat16, float32, float64, int32 and int64 arrays; got "
-      << DTypeName(out.dtype());
-  const int dev = out.dev();
-  if (op != kEwFill) {
-    KV_CHECK(a.on_gpu() && a.dev() == dev) << "all operands must be on the same GPU";
-    KV_CHECK(a.stype() == kDefaultStorage)
-        << "elementwise operators take dense arrays only; an input is not dense (default storage)";
-    KV_CHECK_EQ(a.Size(), out.Size()) << "elementwise shape mismatch";
-    KV_CHECK_EQ(a.dtype(), out.dtype()) << "elementwise dtype mismatch";
-  }
-  if (b) {
-    KV_CHECK(b->on_gpu() && b->dev() == dev) << "all operands must be on the same GPU";
-    KV_CHECK(b->stype() == kDefaultStorage)
-        << "elementwise operators take dense arrays only; an input is not dense (default storage)";
-    KV_CHECK_EQ(b->Size(), out.Size()) << "elementwise shape mismatch";
-    KV_CHECK_EQ(b->dtype(), out.dtype()) << "elementwise dtype mismatch";
-  }
-  LaneOp lop(dev);
-  if (op != kEwFill) lop.Read(a);
-  if (b) lop.Read(*b);
-  lop.Write(out);
-  LaunchElementwise(op, out.dtype(), out.data(), op == kEwFill ? nullptr : a.data(),
-                    b ? b->data() : nullptr, scalar, out.Size(), lop.stream());
-  Engine::Get()->CountLaunch("elementwise", 0);
-  lop.Issue();
 }
 
 // rescale_grad and clip_gradient, which every operator call parses first (InvokeOp)

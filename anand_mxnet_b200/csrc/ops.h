@@ -30,8 +30,8 @@ struct OpInfo {
 // variant bits of the operators that come in plain, mom, mp, multi and preloaded forms
 enum OpFlags { kOpMom = 1, kOpMp = 2, kOpMulti = 4, kOpPreloaded = 8 };
 
-// each family's operators: ops.cc, multi_ops.cc, update_ops.cc
-extern const std::vector<OpInfo> kCoreOps, kMultiTensorOps, kUpdateOps;
+// each family's operators: ops.cc, multi_ops.cc, update_ops.cc, arith_ops.cc
+extern const std::vector<OpInfo> kCoreOps, kMultiTensorOps, kUpdateOps, kArithOps;
 
 // nullptr when the operator is not registered
 const OpInfo* FindOp(const std::string& name);
@@ -45,6 +45,12 @@ NDArray OutOr(std::vector<NDArray>* outputs, size_t i, const std::vector<int64_t
               int dtype);
 // the front-end passes out=weight; a distinct out receives the weight first (then updated in place)
 NDArray InPlace(const std::vector<NDArray>& in, size_t widx, std::vector<NDArray>* outputs, size_t oidx);
+
+// out = op(a[, b], scalar[, scalar2]) through LaunchElementwise (an EwOp code) on out's GPU, after
+// checking that every operand is a dense array on that GPU with out's size and dtype. A failed
+// check throws before anything is enqueued.
+void Elementwise(int op, const NDArray& a, const NDArray* b, double scalar, const NDArray& out,
+                 double scalar2 = 0.0);
 
 // Device copies of the descriptor tables an operator call builds from its operands, kept per
 // operand list so that a repeated call uploads nothing. The key holds everything the tables were

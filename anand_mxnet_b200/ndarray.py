@@ -244,6 +244,12 @@ class NDArray(object):
     def __imul__(self, other):
         return self._binary(other, '_mul', '_mul_scalar', out=self)
 
+    def __truediv__(self, other):
+        return self._binary(other, 'broadcast_div', '_div_scalar')
+
+    def __itruediv__(self, other):
+        return self._binary(other, 'broadcast_div', '_div_scalar', out=self)
+
     def __getitem__(self, key):
         """a[b:e] on the first axis: a view sharing memory (MXNDArraySlice, ndarray.py:_slice)"""
         if isinstance(key, int):
@@ -576,6 +582,14 @@ lamb_update_phase2 = _op('lamb_update_phase2')
 mp_lamb_update_phase1 = _op('mp_lamb_update_phase1')
 mp_lamb_update_phase2 = _op('mp_lamb_update_phase2')
 sqrt = _op('sqrt')
+# the arithmetic of the reference's Adamax, Nadam and AdaDelta optimizers (GPU arrays of one shape;
+# no broadcasting): maximum(lhs, rhs) of two arrays, abs(data), clip(data, a_min, a_max)
+maximum = _op('broadcast_maximum')
+abs = _op('abs')  # noqa: A001  (mx.nd.abs, as the reference names it)
+
+
+def clip(data, a_min, a_max, out=None):
+    return _invoke('clip', [data], out=out, a_min=a_min, a_max=a_max)
 
 
 def norm(data, out=None):
