@@ -544,6 +544,31 @@ void KVStore::PushImpl(const std::vector<int>& keys, const std::vector<NDArray>&
   std::vector<DenseOp> fused, pulls;
   std::set<int> pushed;
   const bool callback = updater_ != nullptr && !opt_.enabled;
+  // 2-bit compression quantises a key's values before the per-key checks below, and every
+  // quantise moves its value's residual: check every compressed key of the call first, so that a
+  // refused call leaves all residuals where they were (and no kernel reads a value as float32
+  // that is not one)
+  if (gc_type_ == "2bit") {
+    for (size_t i = 0; i < uniq.size(); ++i) {
+      const std::vector<NDArray>& srcs = grouped[i];
+      if (srcs[0].stype() != kDefaultStorage) continue;
+      const KeyEntry& e = Entry(uniq[i]);
+      KV_CHECK_EQ(e.stype, kDefaultStorage)
+          << "key " << e.key << " was initialised row_sparse but a dense value was pushed";
+      KV_CHECK_EQ(e.dtype, kFloat32) << "2-bit gradient compression needs float32 gradients";
+      if (dist_) {
+        KV_CHECK_EQ(srcs.size(), 1u) << "one-rank-per-GPU store: push one value per key and rank";
+      } else {
+        KV_CHECK(srcs.size() <= static_cast<size_t>(kMaxSrc))
+            << "at most " << kMaxSrc << " values per key and push";
+      }
+      for (auto& s : srcs) {
+        KV_CHECK_EQ(s.stype(), kDefaultStorage) << "mixed storage types in push";
+        KV_CHECK_EQ(s.Size(), e.size) << "push: shape mismatch for key " << e.key;
+        KV_CHECK_EQ(s.dtype(), e.dtype) << "push: dtype mismatch for key " << e.key;
+      }
+    }
+  }
   // 2-bit compression in a peer group: all dense keys of the call are quantised, exchanged and
   // decoded in one batch (two cross-rank barriers per call, not per key); their merged gradients
   // are identical on every rank, so the rest of the push is a local, one-source launch
@@ -556,7 +581,6 @@ void KVStore::PushImpl(const std::vector<int>& keys, const std::vector<NDArray>&
     for (size_t i = 0; i < uniq.size(); ++i) {
       if (grouped[i][0].stype() != kDefaultStorage) continue;
       KeyEntry& e = Entry(uniq[i]);
-      for (auto& s : grouped[i]) KV_CHECK_EQ(s.Size(), e.size) << "push: shape mismatch for key " << e.key;
       es.push_back(&e);
       vals.push_back(grouped[i]);
       which.push_back(i);
@@ -577,7 +601,6 @@ void KVStore::PushImpl(const std::vector<int>& keys, const std::vector<NDArray>&
     if (gc_type_ == "2bit" && !gc_group && srcs[0].stype() == kDefaultStorage) {
       // CommDevice::Reduce -> ReduceCompressed (comm.h:507-509): quantise every value with its
       // residual, decode + sum on the owner; the optimizer then sees that merged gradient
-      for (auto& s : srcs) KV_CHECK_EQ(s.Size(), e.size) << "push: shape mismatch for key " << e.key;
       NDArray merged = CompressedReduce(e, srcs);
       srcs.assign(1, merged);
     }

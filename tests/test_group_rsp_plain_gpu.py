@@ -108,9 +108,20 @@ def _worker(rank, world, port, q):
         model.set_optimizer('sgd', lr=0.1, momentum=0.9, wd=1e-4, rescale_grad=1.0 / world)
         res = [[np.zeros(int(np.prod(s)), np.float32) for _ in range(world)] for s in shapes]
         outs = [mx.nd.empty(s, ctx) for s in shapes]
-        for step in range(3):
+        for step in range(4):
             def grad(r, k):
                 return np.random.default_rng(4000 + 100 * step + 10 * r + k).uniform(-0.4, 0.4, shapes[k]).astype(np.float32)
+            if step == 3:
+                # a float16 value on the last key: every rank refuses the call before any key's
+                # residual moves, so this step still follows the trajectory that never saw it
+                bad = [mx.nd.array(grad(rank, k), ctx) for k in keys[:-1]]
+                bad.append(mx.nd.array(grad(rank, keys[-1]).astype(np.float16), ctx, 'float16'))
+                try:
+                    kv.pushpull(keys, bad, out=outs)
+                    errors.append("2bit: a float16 value on a float32 key was accepted")
+                except mx.MXNetError as e:
+                    if "push: dtype mismatch for key %d" % keys[-1] not in str(e):
+                        errors.append("2bit: unexpected refusal %s" % e)
             kv.pushpull(keys, [mx.nd.array(grad(rank, k), ctx) for k in keys], out=outs)
             for k, s in enumerate(shapes):
                 n = int(np.prod(s))
