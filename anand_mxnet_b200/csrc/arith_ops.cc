@@ -10,8 +10,11 @@
 //   abs                                             tensor/elemwise_unary_op_basic.cc:707; mshadow_op.h:545
 //   clip                                            tensor/matrix_op.cc:657-700, matrix_op-inl.h:1593-1617
 //
-// Operands of one shape only: the optimizers never broadcast, and a shape that would is refused.
-// Integer division is refused, since the reference's integer arithmetic traps on a zero divisor.
+// Operands of one shape, or an rhs of one value per row: shape lhs.shape[:-1] + (1,) against an lhs
+// of rank 2 or more, the `grad / sqrt(history + eps)` of the reference's GroupAdaGrad (contrib.py:
+// 94-100). Every other broadcast is refused. Integer division is refused, since the reference's
+// integer arithmetic traps on a zero divisor.
+#include <algorithm>
 #include <sstream>
 
 #include "kernels.h"
@@ -36,17 +39,26 @@ void RefuseIntegerDivision(const OpInfo& op, const NDArray& a) {
       << "); divide float16, bfloat16, float32 or float64 arrays";
 }
 
+// rhs's shape is lhs's with its last axis 1, lhs of rank 2 or more
+bool RowOperand(const std::vector<int64_t>& lhs, const std::vector<int64_t>& rhs) {
+  return lhs.size() >= 2 && rhs.size() == lhs.size() && rhs.back() == 1 &&
+         std::equal(lhs.begin(), lhs.end() - 1, rhs.begin());
+}
+
 // broadcast_add, broadcast_sub, broadcast_mul, broadcast_div, broadcast_maximum (variant: the kEw*
 // code)
 void Broadcast(const OpInfo& op, const std::vector<NDArray>& in, std::vector<NDArray>* outputs,
                const Params&) {
   KV_CHECK_EQ(in.size(), 2u) << op.name << " expects 2 inputs";
-  KV_CHECK(in[0].shape() == in[1].shape())
+  const bool same = in[0].shape() == in[1].shape();
+  KV_CHECK(same || RowOperand(in[0].shape(), in[1].shape()))
       << op.name << ": operands of shapes " << ShapeText(in[0].shape()) << " and "
-      << ShapeText(in[1].shape()) << " would broadcast; only operands of equal shapes are supported";
+      << ShapeText(in[1].shape()) << " would broadcast; only operands of equal shapes are supported, "
+      << "or an rhs of shape lhs.shape[:-1] + (1,)";
   if (op.variant == kEwDiv) RefuseIntegerDivision(op, in[0]);
   NDArray o = OutOr(outputs, 0, in[0].shape(), in[0].ctx(), in[0].dtype());
-  Elementwise(op.variant, in[0], &in[1], 0.0, o);
+  if (same) Elementwise(op.variant, in[0], &in[1], 0.0, o);
+  else ElementwiseRows(op.variant, in[0], in[1], o);
 }
 
 // _div_scalar (its scalar: std::stod, then DType(alpha) in the kernel) and abs (variant: the kEw* code)

@@ -96,13 +96,20 @@ void LaunchDenseFused(const DenseLaunch& p, cudaStream_t stream);
 // converts it once to the array's dtype, as the reference's DType(alpha) / static_cast<DType>(value).
 // kEwClip takes its float bounds a_min, a_max as `scalar`, `scalar2` and compares them with each
 // element as the reference's clip kernel does. kEwDiv and kEwDivScalar divide floating types only.
+// b_row > 0 makes `b` one value per row of b_row elements (b[i / b_row]); 0: b has n elements.
 enum EwOp : int {
   kEwCopy = 0, kEwAdd, kEwSub, kEwMul, kEwAddScalar, kEwMulScalar, kEwFill, kEwSqrt,
-  kEwDiv, kEwMax, kEwDivScalar, kEwAbs, kEwClip
+  kEwDiv, kEwMax, kEwDivScalar, kEwAbs, kEwClip, kEwSquare
 };
 bool ElementwiseDTypeOk(int dtype);
 void LaunchElementwise(int op, int dtype, void* out, const void* a, const void* b, double scalar,
-                       size_t n, cudaStream_t stream, double scalar2 = 0.0);
+                       size_t n, cudaStream_t stream, double scalar2 = 0.0, size_t b_row = 0);
+
+// out[r] = the mean of row r of `in`, `rows` rows of `cols` elements each (cols >= 1): each row
+// folded left to right with red::sum's Kahan step in the dtype, then divided by DType(cols), as the
+// reference's mean over the trailing axis (broadcast_reduce-inl.h:161-175, broadcast_reduce_op.h:
+// 630-633). float16, bfloat16, float32 and float64 (reduce_kernels.cu).
+void LaunchRowMean(int dtype, void* out, const void* in, int64_t rows, int64_t cols, cudaStream_t stream);
 void LaunchCast(void* out, int out_dtype, const void* in, int in_dtype, size_t n, cudaStream_t stream);
 
 // ---- row_sparse (rowsparse_kernels.cu) ----

@@ -83,10 +83,20 @@ template <typename C> __device__ __forceinline__ C Clip(C x, float lo, float hi)
   if (x < lo) return static_cast<C>(lo);
   return x;
 }
+// mshadow_op::square over math::sqr (mshadow_op.h:536, math_functions-inl.h:139-147): float(a) *
+// float(a) for every type but double, then DType(...); an integer square above 2^24 loses bits
+__device__ __forceinline__ float Square(float a) { return __fmul_rn(a, a); }
+__device__ __forceinline__ double Square(double a) { return __dmul_rn(a, a); }
+template <typename I> __device__ __forceinline__ I Square(I a) {
+  const float f = static_cast<float>(a);
+  return static_cast<I>(__fmul_rn(f, f));
+}
 
+// b_row > 0: b holds one value per row of b_row elements, read as b[i / b_row] (the row broadcast
+// of binary_broadcast_kernel with an rhs of shape lhs.shape[:-1] + (1,))
 template <typename T>
 __global__ void ew_kernel(int op, T* out, const T* a, const T* b, double scalar, double scalar2,
-                          size_t n) {
+                          size_t n, size_t b_row) {
   typedef typename Calc<T>::type C;
   const T s = FromDouble<T>(scalar);
   for (size_t i = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; i < n;
@@ -100,18 +110,20 @@ __global__ void ew_kernel(int op, T* out, const T* a, const T* b, double scalar,
       continue;
     }
     const C x = Widen(a[i]);
+    const size_t j = b_row ? i / b_row : i;
     C r;
     switch (op) {
-      case kEwAdd: r = Add(x, Widen(b[i])); break;
-      case kEwSub: r = Sub(x, Widen(b[i])); break;
-      case kEwMul: r = Mul(x, Widen(b[i])); break;
+      case kEwAdd: r = Add(x, Widen(b[j])); break;
+      case kEwSub: r = Sub(x, Widen(b[j])); break;
+      case kEwMul: r = Mul(x, Widen(b[j])); break;
       case kEwAddScalar: r = Add(x, Widen(s)); break;
       case kEwMulScalar: r = Mul(x, Widen(s)); break;
-      case kEwDiv: r = Div(x, Widen(b[i])); break;
-      case kEwMax: r = Max(x, Widen(b[i])); break;
+      case kEwDiv: r = Div(x, Widen(b[j])); break;
+      case kEwMax: r = Max(x, Widen(b[j])); break;
       case kEwDivScalar: r = Div(x, Widen(s)); break;
       case kEwAbs: r = Abs(x); break;
       case kEwClip: r = Clip(x, static_cast<float>(scalar), static_cast<float>(scalar2)); break;
+      case kEwSquare: r = Square(x); break;
       default: r = Sqrt(x); break;  // kEwSqrt
     }
     out[i] = Narrow<T>(r);
@@ -141,9 +153,9 @@ inline int GridFor(size_t n) {
 
 template <typename T>
 void ew_launch(int op, void* out, const void* a, const void* b, double scalar, double scalar2,
-               size_t n, cudaStream_t s) {
+               size_t n, size_t b_row, cudaStream_t s) {
   ew_kernel<T><<<GridFor(n), 256, 0, s>>>(op, static_cast<T*>(out), static_cast<const T*>(a),
-                                          static_cast<const T*>(b), scalar, scalar2, n);
+                                          static_cast<const T*>(b), scalar, scalar2, n, b_row);
 }
 
 template <typename TO>
@@ -170,15 +182,15 @@ bool ElementwiseDTypeOk(int dtype) {
 }
 
 void LaunchElementwise(int op, int dtype, void* out, const void* a, const void* b, double scalar,
-                       size_t n, cudaStream_t stream, double scalar2) {
+                       size_t n, cudaStream_t stream, double scalar2, size_t b_row) {
   if (n == 0) return;
   switch (dtype) {
-    case kFloat32: ew_launch<float>(op, out, a, b, scalar, scalar2, n, stream); break;
-    case kFloat16: ew_launch<__half>(op, out, a, b, scalar, scalar2, n, stream); break;
-    case kBfloat16: ew_launch<__nv_bfloat16>(op, out, a, b, scalar, scalar2, n, stream); break;
-    case kFloat64: ew_launch<double>(op, out, a, b, scalar, scalar2, n, stream); break;
-    case kInt32: ew_launch<int32_t>(op, out, a, b, scalar, scalar2, n, stream); break;
-    case kInt64: ew_launch<int64_t>(op, out, a, b, scalar, scalar2, n, stream); break;
+    case kFloat32: ew_launch<float>(op, out, a, b, scalar, scalar2, n, b_row, stream); break;
+    case kFloat16: ew_launch<__half>(op, out, a, b, scalar, scalar2, n, b_row, stream); break;
+    case kBfloat16: ew_launch<__nv_bfloat16>(op, out, a, b, scalar, scalar2, n, b_row, stream); break;
+    case kFloat64: ew_launch<double>(op, out, a, b, scalar, scalar2, n, b_row, stream); break;
+    case kInt32: ew_launch<int32_t>(op, out, a, b, scalar, scalar2, n, b_row, stream); break;
+    case kInt64: ew_launch<int64_t>(op, out, a, b, scalar, scalar2, n, b_row, stream); break;
     default: KV_FATAL << "elementwise op: unsupported dtype " << DTypeName(dtype);
   }
   KV_CUDA(cudaGetLastError());

@@ -51,7 +51,8 @@ NDArray InPlace(const std::vector<NDArray>& in, size_t widx, std::vector<NDArray
 const OpInfo* FindOp(const std::string& name) {
   static const auto* table = [] {
     auto* m = new std::unordered_map<std::string, const OpInfo*>();
-    for (const std::vector<OpInfo>* family : {&kCoreOps, &kMultiTensorOps, &kUpdateOps, &kArithOps}) {
+    for (const std::vector<OpInfo>* family :
+         {&kCoreOps, &kMultiTensorOps, &kUpdateOps, &kArithOps, &kReduceOps}) {
       for (const OpInfo& op : *family) {
         KV_CHECK(m->emplace(op.name, &op).second) << "operator " << op.name << " is declared twice";
       }
@@ -62,10 +63,13 @@ const OpInfo* FindOp(const std::string& name) {
   return it == table->end() ? nullptr : it->second;
 }
 
+namespace {
+
 // Dense operands only: the kernel walks Size() elements from data(), and a row_sparse array's
-// data() holds only its stored rows. Every check runs before anything is enqueued.
-void Elementwise(int op, const NDArray& a, const NDArray* b, double scalar, const NDArray& out,
-                 double scalar2) {
+// data() holds only its stored rows. Every check runs before anything is enqueued. per_row: b holds
+// one value per row of a's trailing axis.
+void CheckedElementwise(int op, const NDArray& a, const NDArray* b, bool per_row, double scalar,
+                        const NDArray& out, double scalar2) {
   KV_CHECK(out.on_gpu()) << "elementwise operators run on GPU arrays only";
   KV_CHECK(out.stype() == kDefaultStorage)
       << "elementwise operators take dense arrays only; out is not dense (default storage)";
@@ -73,6 +77,11 @@ void Elementwise(int op, const NDArray& a, const NDArray* b, double scalar, cons
       << "elementwise operators take float16, bfloat16, float32, float64, int32 and int64 arrays; got "
       << DTypeName(out.dtype());
   const int dev = out.dev();
+  size_t b_row = 1;
+  if (per_row) {
+    KV_CHECK(!a.shape().empty()) << "a row broadcast needs an operand of rank 1 or more";
+    b_row = static_cast<size_t>(a.shape().back());
+  }
   if (op != kEwFill) {
     KV_CHECK(a.on_gpu() && a.dev() == dev) << "all operands must be on the same GPU";
     KV_CHECK(a.stype() == kDefaultStorage)
@@ -84,7 +93,7 @@ void Elementwise(int op, const NDArray& a, const NDArray* b, double scalar, cons
     KV_CHECK(b->on_gpu() && b->dev() == dev) << "all operands must be on the same GPU";
     KV_CHECK(b->stype() == kDefaultStorage)
         << "elementwise operators take dense arrays only; an input is not dense (default storage)";
-    KV_CHECK_EQ(b->Size(), out.Size()) << "elementwise shape mismatch";
+    KV_CHECK_EQ(b->Size() * b_row, out.Size()) << "elementwise shape mismatch";
     KV_CHECK_EQ(b->dtype(), out.dtype()) << "elementwise dtype mismatch";
   }
   LaneOp lop(dev);
@@ -92,9 +101,21 @@ void Elementwise(int op, const NDArray& a, const NDArray* b, double scalar, cons
   if (b) lop.Read(*b);
   lop.Write(out);
   LaunchElementwise(op, out.dtype(), out.data(), op == kEwFill ? nullptr : a.data(),
-                    b ? b->data() : nullptr, scalar, out.Size(), lop.stream(), scalar2);
+                    b ? b->data() : nullptr, scalar, out.Size(), lop.stream(), scalar2,
+                    per_row ? b_row : 0);
   Engine::Get()->CountLaunch("elementwise", 0);
   lop.Issue();
+}
+
+}  // namespace
+
+void Elementwise(int op, const NDArray& a, const NDArray* b, double scalar, const NDArray& out,
+                 double scalar2) {
+  CheckedElementwise(op, a, b, false, scalar, out, scalar2);
+}
+
+void ElementwiseRows(int op, const NDArray& a, const NDArray& b, const NDArray& out) {
+  CheckedElementwise(op, a, &b, true, 0.0, out, 0.0);
 }
 
 namespace {

@@ -30,8 +30,8 @@ struct OpInfo {
 // variant bits of the operators that come in plain, mom, mp, multi and preloaded forms
 enum OpFlags { kOpMom = 1, kOpMp = 2, kOpMulti = 4, kOpPreloaded = 8 };
 
-// each family's operators: ops.cc, multi_ops.cc, update_ops.cc, arith_ops.cc
-extern const std::vector<OpInfo> kCoreOps, kMultiTensorOps, kUpdateOps, kArithOps;
+// each family's operators: ops.cc, multi_ops.cc, update_ops.cc, arith_ops.cc, reduce_ops.cc
+extern const std::vector<OpInfo> kCoreOps, kMultiTensorOps, kUpdateOps, kArithOps, kReduceOps;
 
 // nullptr when the operator is not registered
 const OpInfo* FindOp(const std::string& name);
@@ -51,6 +51,9 @@ NDArray InPlace(const std::vector<NDArray>& in, size_t widx, std::vector<NDArray
 // check throws before anything is enqueued.
 void Elementwise(int op, const NDArray& a, const NDArray* b, double scalar, const NDArray& out,
                  double scalar2 = 0.0);
+// out = op(a, b) for a binary EwOp code, where b holds one value per row of a's trailing axis
+// (b[i / a.shape().back()]), with Elementwise's checks; b's size must be out's over that row length
+void ElementwiseRows(int op, const NDArray& a, const NDArray& b, const NDArray& out);
 
 // Device copies of the descriptor tables an operator call builds from its operands, kept per
 // operand list so that a repeated call uploads nothing. The key holds everything the tables were

@@ -265,6 +265,9 @@ class NDArray(object):
     def norm(self):
         return norm(self)
 
+    def mean(self, axis=None, keepdims=False, exclude=False, out=None):
+        return mean(self, axis=axis, keepdims=keepdims, exclude=exclude, out=out)
+
     def __setitem__(self, key, value):
         if not (isinstance(key, slice) and key == slice(None)):
             raise MXNetError('only full-slice assignment (a[:] = v) is supported')
@@ -590,6 +593,16 @@ abs = _op('abs')  # noqa: A001  (mx.nd.abs, as the reference names it)
 
 def clip(data, a_min, a_max, out=None):
     return _invoke('clip', [data], out=out, a_min=a_min, a_max=a_max)
+
+
+# the two operators the dense-gradient branches of the reference's AdaGrad and GroupAdaGrad add:
+# square(data) on every dtype, and the mean over the last axis of a float array of rank 2 or more
+# (axis=-1 or its positive index; any other axis is refused)
+square = _op('square')
+
+
+def mean(data, axis=None, keepdims=False, exclude=False, out=None):
+    return _invoke('mean', [data], out=out, axis=axis, keepdims=keepdims, exclude=exclude)
 
 
 def norm(data, out=None):

@@ -1,0 +1,28 @@
+# TEST INFRASTRUCTURE ONLY (see oracle/README.md).
+#
+#   make -f oracle/dense_adagrad.mk -> oracle/_ref/libmxref_dense_adagrad.so: square, mean over
+#   ReduceAxesParam and the row broadcast of the five binary operators, as the dense-gradient
+#   branches of the reference's AdaGrad and GroupAdaGrad call them (ref_dense_adagrad.cc, which
+#   includes ref_ndarray_ops.cc), compiled from src/operator/ where they lie under $(REF). Same flags
+#   as oracle/arith_ops.mk (the reference's CPU build); outputs only into oracle/_ref/ (git-ignored).
+REF ?= /root/reference
+CXX := g++
+HERE := $(dir $(abspath $(lastword $(MAKEFILE_LIST))))
+
+REF_FLAGS = -std=c++11 -O3 -msse3 -funroll-loops -fopenmp -fPIC -shared -w -DNDEBUG \
+  -DMSHADOW_USE_CUDA=0 -DMSHADOW_USE_CBLAS=0 -DMSHADOW_USE_MKL=0 -DMXNET_USE_CUDA=0 \
+  -DMXNET_USE_OPENCV=0 -DMXNET_USE_MKLDNN=0 -DMXNET_USE_LAPACK=0 -DDMLC_USE_CXX11=1 \
+  -DMSHADOW_IN_CXX11=1 -DDMLC_LOG_STACK_TRACE=0 -DMSHADOW_USE_F16C=0 \
+  -I$(REF)/include -I$(REF)/src -I$(REF)/3rdparty/mshadow -I$(REF)/3rdparty/dmlc-core/include \
+  -I$(REF)/3rdparty/tvm/nnvm/include -I$(REF)/3rdparty/tvm/include -I$(REF)/3rdparty/dlpack/include
+
+ref_dense_adagrad: $(HERE)_ref/libmxref_dense_adagrad.so
+
+$(HERE)_ref/libmxref_dense_adagrad.so: $(HERE)ref_dense_adagrad.cc $(HERE)ref_ndarray_ops.cc
+	@if [ -f "$(REF)/src/operator/tensor/broadcast_reduce_op.h" ]; then \
+	  mkdir -p $(HERE)_ref && \
+	  $(CXX) $(REF_FLAGS) -I$(HERE) -Wl,--no-undefined -o $@ $< && \
+	  echo "built oracle/_ref/libmxref_dense_adagrad.so from $(REF)"; \
+	else echo "reference tree $(REF) not present: keeping any prebuilt oracle/_ref/libmxref_dense_adagrad.so"; fi
+
+.PHONY: ref_dense_adagrad
