@@ -181,7 +181,16 @@ __device__ __forceinline__ void process(const KeyDesc& k, uint32_t off, uint32_t
         }
       }
       // ---- optimizer step
-      if (OPT != kOptAssign) {
+      if (OPT == kOptTest && sizeof(T) == 2) {
+        // weight[:] += grad * rescale_grad on a 16-bit key: _mul_scalar then _plus, each rounding
+        // to T as mshadow's half arithmetic does, with the scalar cast to T first (a Test key never
+        // carries an fp32 master)
+        const float r = Cvt<T>::round(h.rescale);
+#pragma unroll
+        for (int j = 0; j < V; ++j) {
+          acc[u][j] = Cvt<T>::round(__fadd_rn(wv[u][j], Cvt<T>::round(__fmul_rn(acc[u][j], r))));
+        }
+      } else if (OPT != kOptAssign) {
 #pragma unroll
         for (int j = 0; j < V; ++j) acc[u][j] = step<OPT>(wv[u][j], acc[u][j], s1[u][j], s2[u][j], has_mom, h);
         if ((OPT == kOptSGD && has_mom) || OPT == kOptAdam) IO<float, V>::st(k.s1 + base[u], s1[u]);

@@ -243,6 +243,28 @@ void RunRspUpdate(int opt, const NDArray& w, const NDArray& g, const NDArray& s1
   op.Issue();
 }
 
+// Weight dtypes, checked before InPlace copies a weight into a distinct out. The fused step computes
+// in float32 and rounds once on store. The reference's non-mp forms compute in the weight's own
+// type and round after every operation (optimizer_op-inl.h:225-250, 410-418), so they take float32
+// weights only; 16-bit weights go through the mp forms, which keep a float32 master copy.
+void CheckWeightDTypes(const OpInfo& op, const std::vector<NDArray>& in, int num, int stride, bool mp) {
+  for (int i = 0; i < num; ++i) {
+    const int dt = in[static_cast<size_t>(i) * stride].dtype();
+    if (mp) {
+      KV_CHECK(dt == kFloat32 || dt == kFloat16 || dt == kBfloat16)
+          << op.name << " takes float32, float16 or bfloat16 weights; weight " << i << " is "
+          << DTypeName(dt);
+    } else if (dt != kFloat32) {
+      std::string mp_form = op.name;
+      const size_t at = mp_form.find("sgd");
+      mp_form = at == std::string::npos ? "a float32 master copy (multi_precision=True)"
+                                        : mp_form.insert(at, "mp_");
+      KV_FATAL << op.name << " takes float32 weights; weight " << i << " is " << DTypeName(dt)
+               << " (float16 / bfloat16 weights need " << mp_form << ")";
+    }
+  }
+}
+
 // rescale_grad and clip_gradient, which every operator call parses first (InvokeOp)
 DenseLaunch GradScalars(const Params& p) {
   DenseLaunch S;
@@ -260,6 +282,7 @@ void SgdAdam(const OpInfo& op, const std::vector<NDArray>& in, std::vector<NDArr
   const bool adam = kind == kOptAdam;
   const size_t nin = adam ? 4 : (mom ? 3 : 2);
   KV_CHECK_EQ(in.size(), nin) << op.name << " expects " << nin << " inputs";
+  CheckWeightDTypes(op, in, 1, 0, false);
   NDArray w = InPlace(in, 0, outputs, 0);
   if (in[1].stype() == kRowSparseStorage) {
     RspUpdateLaunch L;
@@ -306,6 +329,7 @@ void MpSgd(const OpInfo& op, const std::vector<NDArray>& in, std::vector<NDArray
   DenseLaunch S = GradScalars(p);
   const bool mom = op.variant == kOptSGD;
   KV_CHECK_EQ(in.size(), mom ? 4u : 3u) << op.name << ": wrong number of inputs";
+  CheckWeightDTypes(op, in, 1, 0, true);
   AdhocKey k;
   k.w = InPlace(in, 0, outputs, 0);
   k.g = in[1];
@@ -339,6 +363,7 @@ void MultiSgd(const OpInfo& op, const std::vector<NDArray>& in, std::vector<NDAr
     KV_CHECK_EQ(static_cast<int>(lrs.size()), num) << n << ": len(lrs) != num_weights";
     KV_CHECK_EQ(static_cast<int>(wds.size()), num) << n << ": len(wds) != num_weights";
   }
+  CheckWeightDTypes(op, in, num, stride, mp);
   S.momentum = GetF(p, "momentum", 0.f);
   std::vector<AdhocKey> keys(num);
   for (int i = 0; i < num; ++i) {

@@ -240,33 +240,38 @@ def test_fused_test_optimizer(mx):
                shapes=[(4, 4), (100, 100), (2000, 2000)], rng=rng)
 
 
-@pytest.mark.parametrize("optname", ['sgd', 'adam', 'test'])
-def test_callback_route_equals_fused_route(mx, optname, monkeypatch):
+@pytest.mark.parametrize("optname,dtype", [
+    pytest.param('sgd', np.float32, id='sgd'), pytest.param('adam', np.float32, id='adam'),
+    pytest.param('test', np.float32, id='test'), pytest.param('sgd', np.float16, id='sgd-float16'),
+    pytest.param('adam', np.float16, id='adam-float16')])
+def test_callback_route_equals_fused_route(mx, optname, dtype, monkeypatch):
     """The reference's route (store -> Python Updater -> optimizer operators) and the fused route
-    must agree bit-for-bit, including update counts and Adam's bias-corrected lr."""
+    must agree bit-for-bit, including update counts and Adam's bias-corrected lr. On float16 keys
+    both keep float32 master weights (multi_precision=True)."""
     results = []
+    mp = dtype != np.float32
     for fused in ('1', '0'):
         monkeypatch.setenv('B200KV_FUSED_OPTIMIZER', fused)
         rng = np.random.default_rng(10)
         kv = mx.kv.create('device')
         shapes = SHAPES[:4]
         for k, s in enumerate(shapes):
-            kv.init(k, mx.nd.array(rnd(rng, s), mx.gpu(0)))
+            kv.init(k, mx.nd.array(rnd(rng, s), mx.gpu(0), dtype))
         # objects of the reference's optimizer classes (tests/compat mirror): the store fuses SGD /
         # Adam natively, or -- B200KV_FUSED_OPTIMIZER=0 -- calls their own update() back per key
         from compat import mxnet_optimizer as mxopt
         if optname == 'sgd':
-            opt = mxopt.SGD(learning_rate=0.05, momentum=0.9, wd=1e-3, rescale_grad=0.5)
+            opt = mxopt.SGD(learning_rate=0.05, momentum=0.9, wd=1e-3, rescale_grad=0.5, multi_precision=mp)
         elif optname == 'adam':
-            opt = mxopt.Adam(learning_rate=2e-3, wd=0.02, rescale_grad=0.25)
+            opt = mxopt.Adam(learning_rate=2e-3, wd=0.02, rescale_grad=0.25, multi_precision=mp)
         else:   # dmlc::stof and std::stod-then-float parse this rescale_grad differently
             opt = mxopt.Test(rescale_grad=1.2345e-05)
         kv.set_optimizer(opt)
         assert (kv._fused is not None) == (fused == '1')
-        outs = [mx.nd.empty(s, mx.gpu(0)) for s in shapes]
+        outs = [mx.nd.empty(s, mx.gpu(0), dtype) for s in shapes]
         for _ in range(3):
             for k, s in enumerate(shapes):
-                kv.push(k, [mx.nd.array(rnd(rng, s), mx.gpu(0)) for _ in range(3)])
+                kv.push(k, [mx.nd.array(rnd(rng, s), mx.gpu(0), dtype) for _ in range(3)])
                 kv.pull(k, out=outs[k])
         results.append([o.asnumpy() for o in outs])
     for a, b in zip(*results):
