@@ -48,6 +48,26 @@ NDArray InPlace(const std::vector<NDArray>& in, size_t widx, std::vector<NDArray
   return o;
 }
 
+const char* StypeName(int stype) { return stype == kRowSparseStorage ? "row_sparse" : "default"; }
+
+void ZeroFillEmptyRspStates(const std::vector<NDArray>& states, int64_t rows, const char* launch_name) {
+  std::vector<const NDArray*> fill;
+  for (const NDArray& a : states) {
+    if (!a.is_none() && a.stype() == kRowSparseStorage && a.nnr() == 0) fill.push_back(&a);
+  }
+  if (fill.empty()) return;
+  for (const NDArray* a : fill) a->CheckAndAllocRows(rows);
+  LaneOp lop(fill[0]->dev());
+  for (const NDArray* a : fill) lop.Write(*a);
+  for (const NDArray* a : fill) {
+    const size_t row_bytes = a->RowLength() * DTypeSize(a->dtype());
+    KV_CUDA(cudaMemsetAsync(a->data(), 0, static_cast<size_t>(rows) * row_bytes, lop.stream()));
+    LaunchFillRowIds(a->row_ids(), rows, lop.stream());
+    Engine::Get()->CountLaunch(launch_name, static_cast<uint64_t>(rows) * (row_bytes + 8));
+  }
+  lop.Issue();
+}
+
 const OpInfo* FindOp(const std::string& name) {
   static const auto* table = [] {
     auto* m = new std::unordered_map<std::string, const OpInfo*>();
@@ -220,13 +240,13 @@ void RunAdhoc(int opt, std::vector<AdhocKey>& keys, const DenseLaunch& scalars,
   op.Issue();
 }
 
-// lazy row_sparse gradient: update only the rows listed (optimizer_op-inl.h:452-565,803-876,1410-1470)
+// lazy row_sparse gradient: update only the rows listed (optimizer_op-inl.h:452-565,803-876,1410-1470).
+// w is dense, or row_sparse with every row (SgdAdamRspWeight has checked it): either way its values
+// are the row-major table, addressed by the gradient's row ids.
 void RunRspUpdate(int opt, const NDArray& w, const NDArray& g, const NDArray& s1, const NDArray& s2,
                   RspUpdateLaunch L) {
   KV_CHECK(w.on_gpu() && g.on_gpu() && w.dev() == g.dev()) << "all operands must be on the same GPU";
   KV_CHECK_EQ(w.dtype(), kFloat32) << "row_sparse optimizer updates are float32";
-  KV_CHECK_EQ(w.stype(), kDefaultStorage) << "row_sparse weights with row_sparse gradients: the "
-                                          << "store keeps sparse-updated weights dense";
   if (!g.storage_initialized()) return;  // all-zero gradient: lazy update touches nothing
   LaneOp op(w.dev());
   op.Read(g).Write(w).Write(s1).Write(s2);
@@ -273,7 +293,59 @@ DenseLaunch GradScalars(const Params& p) {
   return S;
 }
 
-// sgd_update, sgd_mom_update, adam_update (variant: the kOpt* kernel code), dense or row_sparse grad
+// sgd_update, sgd_mom_update and adam_update on a row_sparse weight (SGDUpdateEx, SGDMomUpdateEx,
+// AdamUpdateEx: optimizer_op-inl.h:548-565, 972-1004, 1531-1564), float32 only:
+//   (row_sparse weight, row_sparse grad[, row_sparse states])  lazy_update: lazy, else standard
+//   (row_sparse weight, row_sparse grad, dense states)         standard, whatever lazy_update says
+// The weight holds every row, so its values are the row-major table and the dense weight's kernels
+// serve it. A row_sparse state holds every row, or none yet: then it is zero-filled first, in both
+// forms and even when the gradient is empty. Every check runs before anything is enqueued.
+void SgdAdamRspWeight(const OpInfo& op, const std::vector<NDArray>& in, std::vector<NDArray>* outputs,
+                      RspUpdateLaunch L, bool lazy) {
+  const NDArray& w = in[0];
+  const NDArray& g = in[1];
+  const int kind = op.variant;
+  if (in.size() > 2 && in[2].stype() == kDefaultStorage) lazy = false;  // StdOptStorageType (:912-917)
+  KV_CHECK(!w.shape().empty()) << op.name << ": the weight needs at least one dimension";
+  const int64_t rows = w.shape()[0];
+  for (const NDArray& a : in) {
+    KV_CHECK(a.on_gpu() && a.dev() == w.dev()) << op.name << ": all operands must be on the same GPU";
+    KV_CHECK_EQ(a.dtype(), kFloat32) << "row_sparse optimizer updates are float32";
+    KV_CHECK(a.shape() == w.shape()) << op.name << ": weight / grad / state shape mismatch";
+  }
+  // CheckAllRowsPresent (operator_common.h:500-511) under the reference's function names
+  // (optimizer_op-inl.h:541, 859, 958, 1472, 1523)
+  const char* func = kind == kOptSGDSingle ? "SGDUpdate"
+                     : kind == kOptSGD     ? "SGDMomUpdate"
+                     : lazy                ? "AdamUpdate"
+                                           : "AdamStdUpdate";
+  KV_CHECK(w.nnr() == rows)
+      << func << " for RowSparse weights is only implemented for RowSparse weights with all rows "
+      << "containing non-zeros. Expects weights.data.shape[0] (" << w.nnr() << ") == weights.shape[0] ("
+      << rows << ").";
+  for (size_t i = 2; i < in.size(); ++i) {
+    KV_CHECK(in[i].stype() != kRowSparseStorage || in[i].nnr() == 0 || in[i].nnr() == rows)
+        << op.name << ": a row_sparse optimizer state must hold every row or none (it holds "
+        << in[i].nnr() << " of " << rows << ")";
+  }
+  // kWriteInplace is expected (optimizer_op-inl.h:497, 818, 1426)
+  KV_CHECK(outputs->size() == 1 && (*outputs)[0].SameStorage(w) && (*outputs)[0].data() == w.data())
+      << op.name << ": out must be the weight itself (kWriteInplace is expected for sparse " << op.name
+      << ")";
+  const std::vector<NDArray> states(in.begin() + 2, in.end());
+  ZeroFillEmptyRspStates(states, rows, "rsp_state_fill");
+  const NDArray s1 = states.size() > 0 ? states[0] : NDArray();
+  const NDArray s2 = states.size() > 1 ? states[1] : NDArray();
+  L.opt = kind;
+  if (lazy) {
+    RunRspUpdate(kind, w, g, s1, s2, L);
+  } else {
+    RunRspStdUpdate(w, g, s1, s2, L);
+  }
+}
+
+// sgd_update, sgd_mom_update, adam_update (variant: the kOpt* kernel code): dense weight with a dense
+// or row_sparse grad and dense states, or a row_sparse weight (SgdAdamRspWeight)
 void SgdAdam(const OpInfo& op, const std::vector<NDArray>& in, std::vector<NDArray>* outputs,
              const Params& p) {
   DenseLaunch S = GradScalars(p);
@@ -283,8 +355,22 @@ void SgdAdam(const OpInfo& op, const std::vector<NDArray>& in, std::vector<NDArr
   const size_t nin = adam ? 4 : (mom ? 3 : 2);
   KV_CHECK_EQ(in.size(), nin) << op.name << " expects " << nin << " inputs";
   CheckWeightDTypes(op, in, 1, 0, false);
-  NDArray w = InPlace(in, 0, outputs, 0);
-  if (in[1].stype() == kRowSparseStorage) {
+  // storage types (SGDUpdateEx, SGDMomUpdateEx, AdamUpdateEx, StdOptStorageType), checked before a
+  // distinct out is written: states share one stype; a dense weight takes dense states, a
+  // row_sparse weight a row_sparse gradient
+  const int wst = in[0].stype();
+  KV_CHECK(outputs->empty() || (*outputs)[0].stype() == wst) << "Inconsistent weight stype and output stype";
+  KV_CHECK(!adam || in[2].stype() == in[3].stype()) << "Inconsistent mean stype and var stype";
+  const int sst = nin > 2 ? in[2].stype() : kDefaultStorage;
+  const bool rsp_g = in[1].stype() == kRowSparseStorage;
+  if (wst != kDefaultStorage || sst != kDefaultStorage) {
+    std::string got;
+    for (const NDArray& a : in) got += std::string(got.empty() ? "" : ", ") + StypeName(a.stype());
+    KV_CHECK(wst == kRowSparseStorage && rsp_g)
+        << op.name << ": storage types (" << got << ") are not supported: row_sparse states need a "
+        << "row_sparse weight, and a row_sparse weight a row_sparse gradient";
+  }
+  auto rsp_launch = [&] {
     RspUpdateLaunch L;
     L.lr = GetF(p, "lr", 0.f);
     L.wd = GetF(p, "wd", 0.f);
@@ -294,6 +380,16 @@ void SgdAdam(const OpInfo& op, const std::vector<NDArray>& in, std::vector<NDArr
     L.beta1 = GetF(p, "beta1", 0.9f);
     L.beta2 = GetF(p, "beta2", 0.999f);
     L.eps = GetF(p, "epsilon", 1e-8f);
+    return L;
+  };
+  if (wst == kRowSparseStorage) {
+    Required(p, "lr", op.name);
+    SgdAdamRspWeight(op, in, outputs, rsp_launch(), GetB(p, "lazy_update", true));
+    return;
+  }
+  NDArray w = InPlace(in, 0, outputs, 0);
+  if (rsp_g) {
+    RspUpdateLaunch L = rsp_launch();
     if (GetB(p, "lazy_update", true)) {
       RunRspUpdate(kind, w, in[1], (mom || adam) ? in[2] : NDArray(), adam ? in[3] : NDArray(), L);
     } else {

@@ -46,6 +46,15 @@ NDArray OutOr(std::vector<NDArray>* outputs, size_t i, const std::vector<int64_t
 // the front-end passes out=weight; a distinct out receives the weight first (then updated in place)
 NDArray InPlace(const std::vector<NDArray>& in, size_t widx, std::vector<NDArray>* outputs, size_t oidx);
 
+// "row_sparse" or "default", for error messages
+const char* StypeName(int stype);
+
+// FillDnsZerosRspImpl (init_op.h:474-487) for optimizer states: every row_sparse array of `states`
+// that holds no rows gets all `rows` rows, zero values and ids 0..rows-1, in one operation on its
+// GPU's lane, so that a kernel can address its rows by table row id. Dense arrays and row_sparse
+// arrays that hold rows are left alone. launch_name is kept by Engine::CountLaunch.
+void ZeroFillEmptyRspStates(const std::vector<NDArray>& states, int64_t rows, const char* launch_name);
+
 // out = op(a[, b], scalar[, scalar2]) through LaunchElementwise (an EwOp code) on out's GPU, after
 // checking that every operand is a dense array on that GPU with out's size and dtype. A failed
 // check throws before anything is enqueued.

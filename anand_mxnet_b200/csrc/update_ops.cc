@@ -61,8 +61,6 @@ float InRange(float v, const char* key, float lo, float hi) {
   return v;
 }
 
-const char* StypeName(int stype) { return stype == kRowSparseStorage ? "row_sparse" : "default"; }
-
 // ftrl_update (FtrlUpdateEx, optimizer_op-inl.h:2291-2314), _sparse_adagrad_update
 // (AdagradStorageType / AdagradUpdateEx, 2480-2501, 2620-2649) and _contrib_group_adagrad_update
 // (GroupAdagradStorageType / GroupAdagradUpdateEx, contrib/optimizer_op-inl.h:67-93, 216-242) with
@@ -144,40 +142,24 @@ void RspUpdateOp(const Spec& spec, const std::vector<NDArray>& in, std::vector<N
            (*outputs)[0].data() == w.data())
       << n << ": out must be the weight itself (kWriteInplace is expected for sparse " << n << ")";
 
-  Engine* eng = Engine::Get();
+  // a state with no rows is zero-filled even when the gradient is empty
+  ZeroFillEmptyRspStates(std::vector<NDArray>(in.begin() + 2, in.end()), rows, spec.launch_name);
+  if (!g.storage_initialized()) return;  // an all-zero gradient changes nothing
   LaneOp lop(w.dev());
-  std::vector<const NDArray*> fill;
-  for (size_t i = 2; i < in.size(); ++i) {
-    if (in[i].stype() == kRowSparseStorage && in[i].nnr() == 0) {
-      in[i].CheckAndAllocRows(rows);
-      fill.push_back(&in[i]);
-    }
-  }
-  const bool update = g.storage_initialized();
-  if (!update && fill.empty()) return;  // an all-zero gradient changes nothing
-  if (update) lop.Read(g);
-  lop.Write(w);
+  lop.Read(g).Write(w);
   for (size_t i = 2; i < in.size(); ++i) lop.Write(in[i]);
-  cudaStream_t st = lop.stream();
-  for (const NDArray* a : fill) {
-    KV_CUDA(cudaMemsetAsync(a->data(), 0, static_cast<size_t>(rows) * a->RowLength() * sizeof(float), st));
-    LaunchFillRowIds(a->row_ids(), rows, st);
-    eng->CountLaunch(spec.launch_name, static_cast<uint64_t>(rows) * (a->RowLength() * 4 + 8));
-  }
-  if (update) {
-    L.w = w.data();
-    L.out = w.data();
-    L.g = g.data();
-    L.gidx = g.row_ids();
-    L.nnr = g.nnr();
-    L.row_len = static_cast<int64_t>(w.RowLength());
-    for (size_t i = 2; i < in.size(); ++i) L.s[i - 2] = static_cast<float*>(in[i].data());
-    LaunchRspRowUpdateOp(L, st);
-    // + 8 B of id per row, and GroupAdaGrad's history value read and written
-    const int64_t per_row = op == kUpdGroupAdaGrad ? 16 : 8;
-    eng->CountLaunch(spec.launch_name,
-                     static_cast<uint64_t>(L.nnr) * (spec.bytes_per_elem * L.row_len + per_row));
-  }
+  L.w = w.data();
+  L.out = w.data();
+  L.g = g.data();
+  L.gidx = g.row_ids();
+  L.nnr = g.nnr();
+  L.row_len = static_cast<int64_t>(w.RowLength());
+  for (size_t i = 2; i < in.size(); ++i) L.s[i - 2] = static_cast<float*>(in[i].data());
+  LaunchRspRowUpdateOp(L, lop.stream());
+  // + 8 B of id per row, and GroupAdaGrad's history value read and written
+  const int64_t per_row = op == kUpdGroupAdaGrad ? 16 : 8;
+  Engine::Get()->CountLaunch(spec.launch_name,
+                             static_cast<uint64_t>(L.nnr) * (spec.bytes_per_elem * L.row_len + per_row));
   lop.Issue();
 }
 

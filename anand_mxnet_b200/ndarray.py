@@ -554,12 +554,18 @@ rmsprop_update = _op('rmsprop_update')
 rmspropalex_update = _op('rmspropalex_update')
 ftml_update = _op('ftml_update')
 ftrl_update = _op('ftrl_update')
-# mx.nd.sparse.*: lazy row updates over the rows of a row_sparse gradient (float32, out must be the
-# weight): ftrl_update on row_sparse weight / grad / z / n (mx.nd.ftrl_update takes the same form
-# from its operands' storage types), adagrad_update on (row_sparse, row_sparse, row_sparse) or
-# (dense, row_sparse, dense) with wd = 0
+# mx.nd.sparse.*: row updates driven by a row_sparse gradient (float32, out must be the weight):
+# ftrl_update on row_sparse weight / grad / z / n (mx.nd.ftrl_update takes the same form from its
+# operands' storage types), adagrad_update on (row_sparse, row_sparse, row_sparse) or (dense,
+# row_sparse, dense) with wd = 0. sgd_update, sgd_mom_update and adam_update are the operators of
+# mx.nd under their sparse names: on a row_sparse weight that holds every row, lazy_update=True
+# moves the gradient's rows and lazy_update=False every row; their states are row_sparse (every
+# row, or none yet: zero-filled first) or dense (the standard form)
 _Sparse.ftrl_update = staticmethod(_op('_sparse_ftrl_update'))
 _Sparse.adagrad_update = staticmethod(_op('_sparse_adagrad_update'))
+_Sparse.sgd_update = staticmethod(_op('sgd_update'))
+_Sparse.sgd_mom_update = staticmethod(_op('sgd_mom_update'))
+_Sparse.adam_update = staticmethod(_op('adam_update'))
 # mx.nd.sparse.zeros_like: the _sparse_zeros_like alias of zeros_like (init_op.cc:153-154)
 _Sparse.zeros_like = staticmethod(_op('_sparse_zeros_like'))
 cast = _op('cast')
