@@ -86,8 +86,7 @@ std::shared_ptr<PackList> BuildPackList(std::vector<std::pair<NDArray, NDArray>>
 void RunPackList(PackList& pl) {
   LaneOp op(pl.lane);
   for (auto& pr : pl.pairs) op.Read(pr.first).Write(pr.second);
-  LaunchPackBulk(static_cast<const PackItem*>(pl.d_items), pl.n_items, pl.total_bytes, op.stream(),
-                 pl.host_io ? 32 : 0);
+  LaunchPackBulk(static_cast<const PackItem*>(pl.d_items), pl.n_items, op.stream(), pl.host_io);
   Engine::Get()->CountLaunch("pack_bulk(tma)", 2 * pl.total_bytes);
   op.Issue();
 }
@@ -100,19 +99,7 @@ bool KVStore::CallSignature(int tag, const std::vector<int>& vkeys, const std::v
                             std::vector<uint64_t>* sig) {
   sig->clear();
   sig->reserve(5 + 3 * vkeys.size() + (okeys ? 3 * okeys->size() : 0));
-  // one-rank-per-GPU calls with host-resident operands are staged through the arena: consecutive
-  // calls alternate between two generations of staging buffers (two cached launches per call
-  // pattern), so step k's transfer out overlaps step k+1's kernel
-  bool host_operand = false;
-  if (dist_) {
-    for (auto& a : values) host_operand = host_operand || (!a.is_none() && !a.on_gpu());
-    if (outs != nullptr) for (auto& a : *outs) host_operand = host_operand || (!a.is_none() && !a.on_gpu());
-  }
-  // (alternating generations overlap more, but the pack kernels and the fused kernel then contend,
-  // so the second generation is opt-in: B200KV_STAGE_DOUBLE=1)
-  static const bool two_gens = std::getenv("B200KV_STAGE_DOUBLE") != nullptr;
-  if (host_operand && two_gens) stage_gen_ ^= 1; else stage_gen_ = 0;
-  sig->push_back(static_cast<uint64_t>(tag) * 2 + static_cast<uint64_t>(stage_gen_));
+  sig->push_back(static_cast<uint64_t>(tag));
   sig->push_back(vkeys.size());
   for (size_t i = 0; i < vkeys.size(); ++i) {
     const NDArray& a = values[i];
@@ -202,14 +189,14 @@ void KVStore::PrepareDense(std::vector<DenseOp>& ops, int opt_kind, bool allow_s
     }
     if (devs.size() >= 2) SetDeviceSet(devs);
   }
-  // ---- 2. placement of every key; host-resident operands get device staging buffers
-  // Launch groups: (dtype, striped?, home, bucket). Host-resident operands are staged through the
-  // GPU; such a group is cut into buckets of ~8 MB of staged bytes so the H2D copy of bucket b+1,
-  // the kernel of bucket b and the D2H copy of bucket b-1 run concurrently on the three lanes.
-  static const size_t kStageBucketBytes = []() {
-    const char* s = std::getenv("B200KV_STAGE_BUCKET_MB");
-    return static_cast<size_t>(s ? std::max(1, std::atoi(s)) : 8) << 20;
-  }();
+  // ---- 2. placement of every key; foreign host memory gets device staging buffers
+  // Launch groups: (dtype, striped?, home, bucket). Arrays in the library's own pinned+mapped host
+  // memory are handed to the kernel as they are (it reads gradients / writes weights over PCIe
+  // itself: one launch, no copies, both PCIe directions busy at once); foreign host memory is
+  // staged through the GPU. A group with staged operands is cut into buckets of ~8 MB of staged
+  // bytes so the H2D copy of bucket b+1, the kernel of bucket b and the D2H copy of bucket b-1 run
+  // concurrently on the three lanes.
+  constexpr size_t kStageBucketBytes = size_t{8} << 20;
   std::map<std::tuple<int, int, int, int>, Prepared> groups;
   std::map<std::tuple<int, int, int>, std::pair<int, size_t>> bucket_of;  // -> (bucket, bytes)
   for (auto& op : ops) {
@@ -231,37 +218,9 @@ void KVStore::PrepareDense(std::vector<DenseOp>& ops, int opt_kind, bool allow_s
     }
     KV_CHECK(op.outs.size() <= static_cast<size_t>(kMaxDst)) << "at most " << kMaxDst << " outs per key";
     const auto gkey = std::make_tuple(e.dtype, e.striped ? 1 : 0, e.striped ? -1 : e.home);
-    // Host-resident operands: arrays in the library's own pinned+mapped memory are handed to the
-    // kernel as they are (it reads gradients / writes weights over PCIe itself: one launch, no
-    // copies, both PCIe directions busy at once); foreign host memory is staged through the GPU.
-    // B200KV_HOST_MODE: zc (default) kernel reads and writes host memory; staged: DMA both ways;
-    // in_dma: gradients by the copy engine, weights written by the kernel; in_tma: gradients by
-    // the TMA pack kernel, weights written by the kernel
-    static const int kHostMode = []() {
-      const char* z = std::getenv("B200KV_HOST_MODE");
-      const std::string m = z ? z : "zc";
-      return m == "staged" ? 0 : m == "in_dma" ? 2 : m == "in_tma" ? 3 : m == "pipe" ? 4 : m == "hybrid" ? 5 : 1;
-    }();
-    // hybrid: arrays of at least B200KV_DMA_MIN_KB go through the copy engines in buckets (DMA in,
-    // fused kernel, DMA out pipelined over the three lanes), the many small ones are read / written
-    // by the kernel itself
-    static const size_t kHybridMin = []() {
-      const char* z = std::getenv("B200KV_DMA_MIN_KB");
-      return static_cast<size_t>(z ? std::max(1, std::atoi(z)) : 1024) << 10;
-    }();
-    // pipe: TMA pack kernels on the two copy lanes move each bucket in / out (one launch per
-    // bucket and direction) while the compute lane runs the fused kernel of the bucket between
-    auto direct_in = [&](const NDArray& a) {
-      return a.on_gpu() || (kHostMode == 1 && a.kernel_visible_host()) ||
-             (kHostMode == 5 && a.kernel_visible_host() && a.ByteSize() < kHybridMin);
-    };
-    auto direct_out = [&](const NDArray& a) {
-      return a.on_gpu() || (kHostMode >= 1 && kHostMode <= 3 && a.kernel_visible_host()) ||
-             (kHostMode == 5 && a.kernel_visible_host() && a.ByteSize() < kHybridMin);
-    };
     size_t staged = 0;
-    for (auto& s : op.srcs) if (!direct_in(s)) staged += s.ByteSize();
-    for (auto& o : op.outs) if (!direct_out(o)) staged += o.ByteSize();
+    for (auto& s : op.srcs) if (!s.kernel_visible()) staged += s.ByteSize();
+    for (auto& o : op.outs) if (!o.kernel_visible()) staged += o.ByteSize();
     auto& bk = bucket_of[gkey];
     if (staged > 0 && bk.second > 0 && bk.second + staged > kStageBucketBytes) {
       ++bk.first;
@@ -272,7 +231,7 @@ void KVStore::PrepareDense(std::vector<DenseOp>& ops, int opt_kind, bool allow_s
     const int stage_dev = e.striped ? devset_[0] : e.home;
     DenseOp dop = op;
     for (size_t i = 0; i < dop.srcs.size(); ++i) {
-      if (!direct_in(dop.srcs[i])) {
+      if (!dop.srcs[i].kernel_visible()) {
         NDArray st = StageSrc(e, i, dop.srcs[i], stage_dev);
         P.stage_in.emplace_back(dop.srcs[i], st);
         dop.srcs[i] = st;
@@ -281,7 +240,7 @@ void KVStore::PrepareDense(std::vector<DenseOp>& ops, int opt_kind, bool allow_s
     for (size_t i = 0; i < dop.outs.size(); ++i) {
       KV_CHECK_EQ(dop.outs[i].Size(), e.size) << "pull: shape mismatch for key " << e.key;
       KV_CHECK_EQ(dop.outs[i].dtype(), e.dtype) << "pull: dtype mismatch for key " << e.key;
-      if (!direct_out(dop.outs[i])) {
+      if (!dop.outs[i].kernel_visible()) {
         NDArray st = StageOut(e, i, dop.outs[i], stage_dev);
         P.stage_out.emplace_back(st, dop.outs[i]);
         dop.outs[i] = st;
@@ -307,11 +266,6 @@ void KVStore::PrepareDense(std::vector<DenseOp>& ops, int opt_kind, bool allow_s
     }
     P.parts.assign(part_set.begin(), part_set.end());
     eng->RequirePeerAccess(P.parts);
-    const char* hm = std::getenv("B200KV_HOST_MODE");
-    if (hm != nullptr && (std::string(hm) == "in_tma" || std::string(hm) == "pipe")) {
-      P.pack_in = BuildPackList(&P.stage_in);
-    }
-    if (hm != nullptr && std::string(hm) == "pipe") P.pack_out = BuildPackList(&P.stage_out);
     out->push_back(std::move(P));
   }
 }
@@ -427,27 +381,20 @@ void KVStore::RunPrepared(Prepared& P) {
       // epoch, start flags only), so a rank whose peers are late -- a checkpoint, an evaluation
       // pass, a slow data loader on one rank -- waits with ONE resident CTA instead of a grid of
       // spinning ones, and the SMs stay free for whatever else its streams have queued.
-      // B200KV_GATE=0 puts the wait back inside the fused kernel.
-      static const bool gate = []() {
-        const char* z = std::getenv("B200KV_GATE");
-        return z == nullptr || z[0] != '0';
-      }();
-      if (gate) {
-        DenseLaunch G;
-        G.signal_pads = L.signal_pads;
-        G.counter = L.counter;
-        G.rank = L.rank;
-        G.world = L.world;
-        G.epoch = L.epoch;
-        G.err_word = L.err_word;
-        G.timeout_ns = L.timeout_ns;
-        G.n_chunks = 0;
-        G.dtype = kFloat32;
-        G.opt = kOptAssign;
-        G.barrier_mask = 1;
-        LaunchDenseFused(G, st);
-        L.barrier_mask = 2;
-      }
+      DenseLaunch G;
+      G.signal_pads = L.signal_pads;
+      G.counter = L.counter;
+      G.rank = L.rank;
+      G.world = L.world;
+      G.epoch = L.epoch;
+      G.err_word = L.err_word;
+      G.timeout_ns = L.timeout_ns;
+      G.n_chunks = 0;
+      G.dtype = kFloat32;
+      G.opt = kOptAssign;
+      G.barrier_mask = 1;
+      LaunchDenseFused(G, st);
+      L.barrier_mask = 2;
     }
     L.keys = static_cast<const KeyDesc*>(pd.d_keys);
     L.chunks = static_cast<const ChunkDesc*>(pd.d_chunks);

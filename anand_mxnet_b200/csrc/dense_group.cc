@@ -121,19 +121,9 @@ void KVStore::PrepareDenseGroup(std::vector<DenseOp>& ops, int opt_kind, std::ve
   KV_CHECK(g != nullptr);
   const int dev = g->dev();
   const bool is_push = opt_kind != kOptPullOnly;
-  // Launch groups by (dtype, bucket). Operands outside this rank's arena (host memory, a
-  // framework's own tensors) are staged by TMA pack launches on the copy lanes. With
-  // B200KV_GROUP_BUCKET_MB=n such a call is cut into buckets of ~n MB of key bytes so that the
-  // transfer in of bucket b+1, the fused kernel of bucket b and the transfer out of bucket b-1
-  // overlap. Off by default: with both PCIe directions busy the (B+1)-stage pipeline has not been
-  // shown to beat one launch per direction, and every bucket also costs a cross-rank barrier (not
-  // measured on H100). Calls whose operands all live in the arena are always ONE launch.
-  static const size_t kBucketBytes = []() {
-    const char* z = std::getenv("B200KV_GROUP_BUCKET_MB");
-    return z ? static_cast<size_t>(std::max(1, std::atoi(z))) << 20 : ~static_cast<size_t>(0) >> 1;
-  }();
-  std::map<std::pair<int, int>, Prepared> groups;
-  std::map<int, std::pair<int, size_t>> bucket_of;  // dtype -> (bucket, bytes in it)
+  // One launch group per dtype. Operands outside this rank's arena (host memory, a framework's own
+  // tensors) are staged through arena buffers around the launch.
+  std::map<int, Prepared> groups;
   auto arena_copy = [&](const NDArray& a) { return a.on_gpu() && a.dev() == dev && g->InArena(a.data()); };
   for (auto& op : ops) {
     KeyEntry& e = *op.e;
@@ -143,19 +133,7 @@ void KVStore::PrepareDenseGroup(std::vector<DenseOp>& ops, int opt_kind, std::ve
         << "one-rank-per-GPU store: at most " << kMaxLocalOut << " pull targets per key per rank";
     if (e.home < 0) EnsureOnDevice(e, dev);
     KV_CHECK_EQ(e.home, dev) << "key " << e.key << " lives on another GPU than this rank's";
-    bool staged = false;
-    for (auto& s : op.srcs) staged = staged || !arena_copy(s);
-    for (auto& o : op.outs) staged = staged || !arena_copy(o);
-    auto& bk = bucket_of[e.dtype];
-    const size_t kbytes = e.size * DTypeSize(e.dtype);
-    if (staged) {
-      if (bk.second > 0 && bk.second + kbytes > kBucketBytes) {
-        ++bk.first;
-        bk.second = 0;
-      }
-      bk.second += kbytes;
-    }
-    Prepared& P = groups[std::make_pair(e.dtype, bk.first)];
+    Prepared& P = groups[e.dtype];
     DenseOp dop = op;
     for (size_t i = 0; i < dop.srcs.size(); ++i) {
       KV_CHECK_EQ(dop.srcs[i].Size(), e.size) << "push: shape mismatch for key " << e.key;
@@ -181,20 +159,18 @@ void KVStore::PrepareDenseGroup(std::vector<DenseOp>& ops, int opt_kind, std::ve
   for (auto& kv : groups) {
     Prepared& P = kv.second;
     P.opt_kind = opt_kind;
-    P.dtype = kv.first.first;
+    P.dtype = kv.first;
     P.is_push = is_push;
     P.group = true;
     P.owners = {dev};
     P.parts = {dev};
     for (auto& op : P.ops) StateOn(*op.e, dev, opt_kind);
     // operands that live outside the IPC arena on this GPU (a framework's own tensors) are packed
-    // into / unpacked from arena staging buffers by one TMA bulk-copy launch each way
-    static const size_t dma_min = []() {
-      const char* z = std::getenv("B200KV_DMA_MIN_KB");
-      return static_cast<size_t>(z ? std::max(0, std::atoi(z)) : 1024) << 10;
-    }();
-    P.pack_in = BuildPackList(&P.stage_in, dma_min);
-    P.pack_out = BuildPackList(&P.stage_out, dma_min);
+    // into / unpacked from arena staging buffers by one pack launch each way; host arrays of 1 MB
+    // and more go to the copy engines instead
+    constexpr size_t kDmaMinBytes = size_t{1} << 20;
+    P.pack_in = BuildPackList(&P.stage_in, kDmaMinBytes);
+    P.pack_out = BuildPackList(&P.stage_out, kDmaMinBytes);
     P.plan = GetPlanGroup(P.ops, opt_kind);
     out->push_back(std::move(P));
   }
@@ -252,9 +228,8 @@ std::shared_ptr<Plan> KVStore::GetPlanGroup(const std::vector<DenseOp>& ops, int
   if (it != plans_.end()) return it->second;
   if (plans_.size() > 256) plans_.clear();
 
-  // ---- collective: first make sure every rank plans the SAME launch (same keys, same cut into
-  // buckets) -- a mismatch would otherwise pair up all-gathers of different sizes or dead-lock the
-  // kernels' barriers
+  // ---- collective: first make sure every rank plans the SAME launch (same keys) -- a mismatch
+  // would otherwise pair up all-gathers of different sizes or dead-lock the kernels' barriers
   {
     uint64_t kh = 0x9b;
     for (auto& op : ops) kh = Mix(kh, static_cast<uint64_t>(op.e->key));
@@ -264,8 +239,7 @@ std::shared_ptr<Plan> KVStore::GetPlanGroup(const std::vector<DenseOp>& ops, int
       KV_CHECK(hdr[3 * r] == hdr[3 * R] && hdr[3 * r + 1] == hdr[3 * R + 1] && hdr[3 * r + 2] == hdr[3 * R + 2])
           << "one-rank-per-GPU store: rank " << r << " issued a different call than rank " << R << " ("
           << hdr[3 * r] << " vs " << hdr[3 * R] << " keys in this launch). Every rank must push / pull "
-          << "the same keys in the same order, with the same kind of arrays (library arrays vs foreign "
-          << "/ host memory decides how a call is cut into buckets)";
+          << "the same keys in the same order";
     }
   }
   // ---- everybody's operand offsets inside its IPC arena

@@ -18,8 +18,6 @@
 // Arithmetic: IEEE fp32 round-to-nearest with NO fused multiply-add (explicit __f*_rn intrinsics;
 // the file is also compiled with -fmad=false) so results are bit-identical to the reference's CPU
 // build (`-O3 -msse3`), i.e. to oracle/kvoracle.c. Expression trees per optimizer are cited below.
-#include <cstdlib>
-
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
 
@@ -105,113 +103,88 @@ template <> struct IO<float, 1> {
   static __device__ __forceinline__ void st(float* p, const float (&x)[1]) { __stcs(p, x[0]); }
 };
 
-// Process U groups of V consecutive elements: group u starts at element off + (v0 + u*kThreads)*V
-// and exists while its vector index is below nvec. EVERY load of every group is issued before the
-// first arithmetic instruction or store (stores to possibly aliasing pointers would otherwise pin
-// the loads of the next group behind them): U x (n_src + 1 + states) 16-byte loads in flight per
-// thread, which is what covers NVLink latency when the sources are peer memory.
-template <typename T, int MAXSRC, int OPT, int V, int U>
-__device__ __forceinline__ void process(const KeyDesc& k, uint32_t off, uint32_t v0, uint32_t nvec,
-                                        int n_src, int n_out, int order, const Hyper& h) {
-  float acc[U][V];
-  float wv[U][V], s1[U][V], s2[U][V];
+// Process V consecutive elements, starting at element off + v*V. EVERY load is issued before the
+// first arithmetic instruction or store: n_src + 1 + states 16-byte loads in flight per thread,
+// which is what covers NVLink latency when the sources are peer memory.
+template <typename T, int MAXSRC, int OPT, int V>
+__device__ __forceinline__ void process(const KeyDesc& k, uint32_t off, uint32_t v, int n_src, int n_out,
+                                        int order, const Hyper& h) {
+  float acc[V];
+  float wv[V], s1[V], s2[V];
   const bool has_mom = k.s1 != nullptr;
   const bool mp = k.w32 != nullptr;
-  uint32_t base[U];
-  bool on[U];
-#pragma unroll
-  for (int u = 0; u < U; ++u) {
-    const uint32_t v = v0 + u * kThreads;
-    on[u] = v < nvec;
-    base[u] = off + v * V;
-  }
+  const uint32_t base = off + v * V;
   if (OPT != kOptPullOnly) {
-    float g[U][MAXSRC][V];
+    float g[MAXSRC][V];
 #pragma unroll
-    for (int u = 0; u < U; ++u) {
-      if (!on[u]) continue;
-#pragma unroll
-      for (int i = 0; i < MAXSRC; ++i) {
-        if (i < n_src) IO<T, V>::ld(static_cast<const T*>(k.src[i]) + base[u], g[u][i]);
-      }
-      if (OPT != kOptAssign) {
-        if (mp) {
-          IO<float, V>::ld(k.w32 + base[u], wv[u]);
-        } else {
-          IO<T, V>::ld(static_cast<const T*>(k.w_in) + base[u], wv[u]);
-        }
-        if ((OPT == kOptSGD && has_mom) || OPT == kOptAdam) IO<float, V>::ld(k.s1 + base[u], s1[u]);
-        if (OPT == kOptAdam) IO<float, V>::ld(k.s2 + base[u], s2[u]);
-      }
+    for (int i = 0; i < MAXSRC; ++i) {
+      if (i < n_src) IO<T, V>::ld(static_cast<const T*>(k.src[i]) + base, g[i]);
     }
-#pragma unroll
-    for (int u = 0; u < U; ++u) {
-      if (!on[u]) continue;
-      // ---- merged gradient in the reference's association; 16-bit dtypes round after every add,
-      // as mshadow's half arithmetic does (3rdparty/mshadow/mshadow/half.h:45-66)
-#pragma unroll
-      for (int j = 0; j < V; ++j) acc[u][j] = g[u][0][j];
-      if (order == kOrderDevice) {
-        // ((g0+g1)+g2)+...   (ndarray_function-inl.h:402-431)
-#pragma unroll
-        for (int i = 1; i < MAXSRC; ++i) {
-          if (i < n_src) {
-#pragma unroll
-            for (int j = 0; j < V; ++j) acc[u][j] = Cvt<T>::round(__fadd_rn(acc[u][j], g[u][i][j]));
-          }
-        }
+    if (OPT != kOptAssign) {
+      if (mp) {
+        IO<float, V>::ld(k.w32 + base, wv);
       } else {
-        // g0 + (((g1+g2)+g3)+g4) + (((g5+..  (comm.h:357-392)
+        IO<T, V>::ld(static_cast<const T*>(k.w_in) + base, wv);
+      }
+      if ((OPT == kOptSGD && has_mom) || OPT == kOptAdam) IO<float, V>::ld(k.s1 + base, s1);
+      if (OPT == kOptAdam) IO<float, V>::ld(k.s2 + base, s2);
+    }
+    // ---- merged gradient in the reference's association; 16-bit dtypes round after every add,
+    // as mshadow's half arithmetic does (3rdparty/mshadow/mshadow/half.h:45-66)
 #pragma unroll
-        for (int i = 1; i < MAXSRC; i += 4) {
-          if (i < n_src) {
-            float t[V];
+    for (int j = 0; j < V; ++j) acc[j] = g[0][j];
+    if (order == kOrderDevice) {
+      // ((g0+g1)+g2)+...   (ndarray_function-inl.h:402-431)
 #pragma unroll
-            for (int j = 0; j < V; ++j) t[j] = g[u][i][j];
+      for (int i = 1; i < MAXSRC; ++i) {
+        if (i < n_src) {
 #pragma unroll
-            for (int q = 1; q < 4; ++q) {
-              if (i + q < MAXSRC && i + q < n_src) {
+          for (int j = 0; j < V; ++j) acc[j] = Cvt<T>::round(__fadd_rn(acc[j], g[i][j]));
+        }
+      }
+    } else {
+      // g0 + (((g1+g2)+g3)+g4) + (((g5+..  (comm.h:357-392)
 #pragma unroll
-                for (int j = 0; j < V; ++j) t[j] = Cvt<T>::round(__fadd_rn(t[j], g[u][i + q][j]));
-              }
+      for (int i = 1; i < MAXSRC; i += 4) {
+        if (i < n_src) {
+          float t[V];
+#pragma unroll
+          for (int j = 0; j < V; ++j) t[j] = g[i][j];
+#pragma unroll
+          for (int q = 1; q < 4; ++q) {
+            if (i + q < MAXSRC && i + q < n_src) {
+#pragma unroll
+              for (int j = 0; j < V; ++j) t[j] = Cvt<T>::round(__fadd_rn(t[j], g[i + q][j]));
             }
-#pragma unroll
-            for (int j = 0; j < V; ++j) acc[u][j] = Cvt<T>::round(__fadd_rn(acc[u][j], t[j]));
           }
+#pragma unroll
+          for (int j = 0; j < V; ++j) acc[j] = Cvt<T>::round(__fadd_rn(acc[j], t[j]));
         }
       }
-      // ---- optimizer step
-      if (OPT == kOptTest && sizeof(T) == 2) {
-        // weight[:] += grad * rescale_grad on a 16-bit key: _mul_scalar then _plus, each rounding
-        // to T as mshadow's half arithmetic does, with the scalar cast to T first (a Test key never
-        // carries an fp32 master)
-        const float r = Cvt<T>::round(h.rescale);
-#pragma unroll
-        for (int j = 0; j < V; ++j) {
-          acc[u][j] = Cvt<T>::round(__fadd_rn(wv[u][j], Cvt<T>::round(__fmul_rn(acc[u][j], r))));
-        }
-      } else if (OPT != kOptAssign) {
-#pragma unroll
-        for (int j = 0; j < V; ++j) acc[u][j] = step<OPT>(wv[u][j], acc[u][j], s1[u][j], s2[u][j], has_mom, h);
-        if ((OPT == kOptSGD && has_mom) || OPT == kOptAdam) IO<float, V>::st(k.s1 + base[u], s1[u]);
-        if (OPT == kOptAdam) IO<float, V>::st(k.s2 + base[u], s2[u]);
-        if (mp) IO<float, V>::st(k.w32 + base[u], acc[u]);
-      }
-      IO<T, V>::st(static_cast<T*>(k.w) + base[u], acc[u]);
     }
+    // ---- optimizer step
+    if (OPT == kOptTest && sizeof(T) == 2) {
+      // weight[:] += grad * rescale_grad on a 16-bit key: _mul_scalar then _plus, each rounding
+      // to T as mshadow's half arithmetic does, with the scalar cast to T first (a Test key never
+      // carries an fp32 master)
+      const float r = Cvt<T>::round(h.rescale);
+#pragma unroll
+      for (int j = 0; j < V; ++j) {
+        acc[j] = Cvt<T>::round(__fadd_rn(wv[j], Cvt<T>::round(__fmul_rn(acc[j], r))));
+      }
+    } else if (OPT != kOptAssign) {
+#pragma unroll
+      for (int j = 0; j < V; ++j) acc[j] = step<OPT>(wv[j], acc[j], s1[j], s2[j], has_mom, h);
+      if ((OPT == kOptSGD && has_mom) || OPT == kOptAdam) IO<float, V>::st(k.s1 + base, s1);
+      if (OPT == kOptAdam) IO<float, V>::st(k.s2 + base, s2);
+      if (mp) IO<float, V>::st(k.w32 + base, acc);
+    }
+    IO<T, V>::st(static_cast<T*>(k.w) + base, acc);
   } else {
-#pragma unroll
-    for (int u = 0; u < U; ++u) {
-      if (on[u]) IO<T, V>::ld(static_cast<const T*>(k.w_in) + base[u], acc[u]);
-    }
+    IO<T, V>::ld(static_cast<const T*>(k.w_in) + base, acc);
   }
   // ---- broadcast to every pull target (peer stores ride NVLink)
-  for (int o = 0; o < n_out; ++o) {
-#pragma unroll
-    for (int u = 0; u < U; ++u) {
-      if (on[u]) IO<T, V>::st(static_cast<T*>(k.out[o]) + base[u], acc[u]);
-    }
-  }
+  for (int o = 0; o < n_out; ++o) IO<T, V>::st(static_cast<T*>(k.out[o]) + base, acc);
 }
 
 // ---- NVLS variant of one fp32 vector: the cross-rank sum happens INSIDE the NVSwitch
@@ -250,58 +223,30 @@ template <> struct MM<1> {
   }
 };
 
-// U groups per thread, every multimem.ld_reduce (and the local weight / state loads) in flight before
-// the first store: a switch-reduced load takes several microseconds to come back, one at a time per
-// thread leaves the links idle most of the time.
-template <int OPT, int V, int U>
-__device__ __forceinline__ void process_nvls(const KeyDesc& k, uint32_t off, uint32_t v0, uint32_t nvec,
-                                             const Hyper& h) {
-  float acc[U][V], wv[U][V], s1[U][V], s2[U][V];
+// every multimem.ld_reduce (and the local weight / state loads) is issued before the first store
+template <int OPT, int V>
+__device__ __forceinline__ void process_nvls(const KeyDesc& k, uint32_t off, uint32_t v, const Hyper& h) {
+  float acc[V], wv[V], s1[V], s2[V];
   const bool has_mom = k.s1 != nullptr;
   float* w = static_cast<float*>(k.w);
-  uint32_t base[U];
-  bool on[U];
-#pragma unroll
-  for (int u = 0; u < U; ++u) {
-    const uint32_t v = v0 + u * kThreads;
-    on[u] = v < nvec;
-    base[u] = off + v * V;
-  }
+  const uint32_t base = off + v * V;
   if (OPT != kOptPullOnly) {
+    MM<V>::ld_reduce(static_cast<const float*>(k.src[kMaxSrc - 1]) + base, acc);
+    if (OPT != kOptAssign) {
+      IO<float, V>::ld(w + base, wv);
+      if ((OPT == kOptSGD && has_mom) || OPT == kOptAdam) IO<float, V>::ld(k.s1 + base, s1);
+      if (OPT == kOptAdam) IO<float, V>::ld(k.s2 + base, s2);
 #pragma unroll
-    for (int u = 0; u < U; ++u) {
-      if (!on[u]) continue;
-      MM<V>::ld_reduce(static_cast<const float*>(k.src[kMaxSrc - 1]) + base[u], acc[u]);
-      if (OPT != kOptAssign) {
-        IO<float, V>::ld(w + base[u], wv[u]);
-        if ((OPT == kOptSGD && has_mom) || OPT == kOptAdam) IO<float, V>::ld(k.s1 + base[u], s1[u]);
-        if (OPT == kOptAdam) IO<float, V>::ld(k.s2 + base[u], s2[u]);
-      }
+      for (int j = 0; j < V; ++j) acc[j] = step<OPT>(wv[j], acc[j], s1[j], s2[j], has_mom, h);
+      if ((OPT == kOptSGD && has_mom) || OPT == kOptAdam) IO<float, V>::st(k.s1 + base, s1);
+      if (OPT == kOptAdam) IO<float, V>::st(k.s2 + base, s2);
     }
-#pragma unroll
-    for (int u = 0; u < U; ++u) {
-      if (!on[u]) continue;
-      if (OPT != kOptAssign) {
-#pragma unroll
-        for (int j = 0; j < V; ++j) acc[u][j] = step<OPT>(wv[u][j], acc[u][j], s1[u][j], s2[u][j], has_mom, h);
-        if ((OPT == kOptSGD && has_mom) || OPT == kOptAdam) IO<float, V>::st(k.s1 + base[u], s1[u]);
-        if (OPT == kOptAdam) IO<float, V>::st(k.s2 + base[u], s2[u]);
-      }
-      IO<float, V>::st(w + base[u], acc[u]);
-    }
+    IO<float, V>::st(w + base, acc);
   } else {
-#pragma unroll
-    for (int u = 0; u < U; ++u) {
-      if (on[u]) IO<float, V>::ld(w + base[u], acc[u]);
-    }
+    IO<float, V>::ld(w + base, acc);
   }
   const int n_mc = static_cast<int>(k.nvls) - 1;
-  for (int o = 0; o < n_mc; ++o) {
-#pragma unroll
-    for (int u = 0; u < U; ++u) {
-      if (on[u]) MM<V>::st(static_cast<float*>(k.out[kMaxDst - 2 + o]) + base[u], acc[u]);
-    }
-  }
+  for (int o = 0; o < n_mc; ++o) MM<V>::st(static_cast<float*>(k.out[kMaxDst - 2 + o]) + base, acc);
 }
 
 struct KernelArgs {
@@ -371,27 +316,23 @@ __device__ __forceinline__ void peer_signal_and_wait(const KernelArgs& a, int ph
   }
 }
 
-template <typename T, int MAXSRC, int OPT, bool NVLS, int UN>
+template <typename T, int MAXSRC, int OPT>
 constexpr int MinBlocks() {
-  if (sizeof(T) != 4 || (NVLS && UN > 1) || MAXSRC > 8) return 1;   // 16-bit packs carry 8 values per load
+  if (sizeof(T) != 4 || MAXSRC > 8) return 1;   // 16-bit packs carry 8 values per load
   if (MAXSRC == 1) return 5;
   const int adam = OPT == kOptAdam ? 1 : 0;                            // two more state vectors
   return (MAXSRC <= 2 ? 5 : 4) - adam;
 }
 
-// NVLS: the instantiation for launches whose sums happen in the NVSwitch (fp32, MAXSRC = 1); UN =
-// groups of V elements per thread with every load in flight before the first store.
-// For local and peer-memory sources one group per thread: the kernel is limited by the link, not by
-// loads in flight, and the registers of a second group cost resident CTAs. The NVLS mode defaults to
-// one group as well; B200KV_NVLS_UNROLL keeps the deeper variants selectable (multi-GPU choices
-// are not measured on H100).
-template <typename T, int MAXSRC, int OPT, bool NVLS, int UN>
+// NVLS: the instantiation for launches whose sums happen in the NVSwitch (fp32, MAXSRC = 1).
+// One group of V elements per thread: for local and peer-memory sources the kernel is limited by
+// the link, not by loads in flight, and the registers of a second group cost resident CTAs.
+template <typename T, int MAXSRC, int OPT, bool NVLS>
 // resident CTAs per SM matter more than registers here (every CTA starts with two dependent
 // descriptor loads): the caps below keep the register budgets of the round-1 kernel (48 / 48 / 64)
-__global__ void __launch_bounds__(kThreads, MinBlocks<T, MAXSRC, OPT, NVLS, UN>())
+__global__ void __launch_bounds__(kThreads, MinBlocks<T, MAXSRC, OPT>())
 dense_fused_kernel(const KernelArgs a) {
   constexpr int V = 16 / sizeof(T);
-  constexpr int U = UN;
   __shared__ KeyDesc sk;
   __shared__ uint32_t s_last;
   if (a.pads != nullptr && (a.barrier_mask & 1)) {
@@ -419,18 +360,16 @@ dense_fused_kernel(const KernelArgs a) {
   const uint32_t nvec = sk.vec_ok ? c.len / V : 0;
   if (NVLS) {
     // (host side: NVLS plans are fp32 and every key of the launch carries multicast addresses)
-    for (uint32_t v = threadIdx.x; v < nvec; v += kThreads * U) process_nvls<OPT, 4, U>(sk, c.off, v, nvec, h);
+    for (uint32_t v = threadIdx.x; v < nvec; v += kThreads) process_nvls<OPT, 4>(sk, c.off, v, h);
     const uint32_t ntail = c.len - nvec * 4;
-    for (uint32_t e = threadIdx.x; e < ntail; e += kThreads) {
-      process_nvls<OPT, 1, 1>(sk, c.off + nvec * 4, e, ntail, h);
-    }
+    for (uint32_t e = threadIdx.x; e < ntail; e += kThreads) process_nvls<OPT, 1>(sk, c.off + nvec * 4, e, h);
   } else {
-    for (uint32_t v = threadIdx.x; v < nvec; v += kThreads * U) {
-      process<T, MAXSRC, OPT, V, U>(sk, c.off, v, nvec, n_src, n_out, a.order, h);
+    for (uint32_t v = threadIdx.x; v < nvec; v += kThreads) {
+      process<T, MAXSRC, OPT, V>(sk, c.off, v, n_src, n_out, a.order, h);
     }
     const uint32_t ntail = c.len - nvec * V;
     for (uint32_t e = threadIdx.x; e < ntail; e += kThreads) {
-      process<T, MAXSRC, OPT, 1, 1>(sk, c.off + nvec * V, e, ntail, n_src, n_out, a.order, h);
+      process<T, MAXSRC, OPT, 1>(sk, c.off + nvec * V, e, n_src, n_out, a.order, h);
     }
   }
   }  // blockIdx.x < n_chunks
@@ -524,27 +463,19 @@ void launch_plain(const DenseLaunch& p, cudaStream_t s) {
   dense_plain_kernel<T><<<grid, kThreads, 0, s>>>(a, p.opt);
 }
 
-template <typename T, int MAXSRC, int OPT, bool NVLS = false, int UN = 1>
+template <typename T, int MAXSRC, int OPT, bool NVLS = false>
 void launch_one(const DenseLaunch& p, cudaStream_t s) {
   KernelArgs a{p.keys, p.chunks, reinterpret_cast<const float2*>(p.hyper), p.lrs, p.wds, p.order, p.momentum,
                p.rescale, p.clip, p.beta1, p.beta2, p.eps, p.signal_pads, p.counter, p.rank, p.world,
                p.epoch, p.n_chunks, p.err_word, p.timeout_ns, p.barrier_mask};
   const int grid = p.n_chunks > 0 ? p.n_chunks : 1;  // a rank with no chunk still joins the barriers
-  dense_fused_kernel<T, MAXSRC, OPT, NVLS, UN><<<grid, kThreads, 0, s>>>(a);
+  dense_fused_kernel<T, MAXSRC, OPT, NVLS><<<grid, kThreads, 0, s>>>(a);
 }
 
 template <typename T, int OPT>
 void launch_src(const DenseLaunch& p, cudaStream_t s) {
   if (p.nvls) {
-    if constexpr (sizeof(T) == 4) {
-      static const int unroll = []() {
-        const char* z = std::getenv("B200KV_NVLS_UNROLL");
-        return z ? std::atoi(z) : 1;
-      }();
-      if (unroll >= 4) return launch_one<T, 1, OPT, true, 4>(p, s);
-      if (unroll >= 2) return launch_one<T, 1, OPT, true, 2>(p, s);
-      return launch_one<T, 1, OPT, true, 1>(p, s);
-    }
+    if constexpr (sizeof(T) == 4) return launch_one<T, 1, OPT, true>(p, s);
     KV_FATAL << "NVLS launches are float32";
   }
   if (OPT == kOptPullOnly || p.max_src <= 1) return launch_one<T, 1, OPT>(p, s);

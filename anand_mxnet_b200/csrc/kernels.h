@@ -339,7 +339,7 @@ void LaunchDequantizeSum2Bit(const uint32_t* const* d_compressed /* device array
 // ---- TMA bulk-copy packing of many small arrays into one fusion buffer (pack_kernels.cu) ----
 constexpr int kPackTileBytes = 16384;  // one TMA bulk copy; items passed to the kernel are <= this
 struct PackItem { const void* src; void* dst; uint64_t bytes; };
-void LaunchPackBulk(const PackItem* d_items, int n_items, uint64_t max_bytes, cudaStream_t stream,
-                    int max_ctas = 0);
+// host_io: the list has a pinned-host side (SM-issued 16-byte copies); otherwise TMA bulk copies
+void LaunchPackBulk(const PackItem* d_items, int n_items, cudaStream_t stream, bool host_io);
 
 }  // namespace b200kv

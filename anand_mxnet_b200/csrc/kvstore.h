@@ -134,8 +134,7 @@ struct PackList {
   int n_items = 0;
   uint64_t total_bytes = 0;
   // engine lane the launch runs on: the compute lane for device-to-device lists; lists with a
-  // pinned-host side run on the H2D / D2H copy lane, so a bucket's transfer in, its fused kernel
-  // and the previous bucket's transfer out overlap (ordering comes from the arrays' dependencies)
+  // pinned-host side run on the H2D / D2H copy lane (ordering comes from the arrays' dependencies)
   int lane = -1;
   bool host_io = false;
   ~PackList();
@@ -293,7 +292,6 @@ class KVStore {
 
   std::string type_;
   bool dist_ = false;         // created inside a one-rank-per-GPU peer group
-  int stage_gen_ = 0;         // staging-buffer generation of the call being prepared / replayed (0 / 1)
   bool nccl_ = false;         // cross-rank sums go through ncclAllReduce (type 'nccl', or no peer memory)
   bool nccl_type_ = false;    // created as 'nccl': dense values only (src/kvstore/kvstore_nccl.h:62-70)
   int rank_ = 0, group_size_ = 1;

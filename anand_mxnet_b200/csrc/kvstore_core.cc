@@ -854,11 +854,7 @@ DevState& KVStore::StateOn(KeyEntry& e, int dev, int opt_kind) {
 
 // Host-resident values (CPU-context NDArrays) take part through per-key staging buffers on a GPU:
 // the reference's 'local' store stages the other way round (GPU -> pinned host, comm.h:146-164).
-// Two generations of staging buffers (stage_gen_): a store whose calls alternate between them lets
-// the transfer out of step k (D2H lane, reads generation g's out buffers) overlap the fused kernel of
-// step k+1 (writes generation 1-g's), instead of the kernel waiting for the drain.
 NDArray KVStore::StageSrc(KeyEntry& e, size_t slot, const NDArray& host_src, int dev) {
-  slot = slot * 2 + stage_gen_;
   if (e.stage_src.size() <= slot) e.stage_src.resize(slot + 1);
   NDArray& st = e.stage_src[slot];
   if (st.is_none() || st.dev() != dev) st = NDArray(e.shape, Context::GPU(dev), e.dtype);
@@ -867,7 +863,6 @@ NDArray KVStore::StageSrc(KeyEntry& e, size_t slot, const NDArray& host_src, int
 }
 
 NDArray KVStore::StageOut(KeyEntry& e, size_t slot, const NDArray&, int dev) {
-  slot = slot * 2 + stage_gen_;
   if (e.stage_out.size() <= slot) e.stage_out.resize(slot + 1);
   NDArray& st = e.stage_out[slot];
   if (st.is_none() || st.dev() != dev) st = NDArray(e.shape, Context::GPU(dev), e.dtype);

@@ -12,8 +12,6 @@
 // moved by the other threads with plain byte loads. Copy-only, HBM-bound: 2 bytes of traffic per
 // byte packed.
 #include <cstdio>
-#include <cstdlib>
-#include <string>
 
 #include "common.h"
 #include "kernels.h"
@@ -161,34 +159,20 @@ __global__ void __launch_bounds__(kLdstThreads) pack_ldst_kernel(const PackItem*
 
 }  // namespace
 
-void LaunchPackBulk(const PackItem* d_items, int n_items, uint64_t, cudaStream_t stream, int max_ctas) {
+void LaunchPackBulk(const PackItem* d_items, int n_items, cudaStream_t stream, bool host_io) {
   if (n_items <= 0) return;
-  if (max_ctas > 0) {
-    // a host-side list (callers pass max_ctas > 0 only for those); B200KV_PACK_MODE=tma keeps the
-    // bulk-copy engine for them
-    static const bool tma_host = []() {
-      const char* z = std::getenv("B200KV_PACK_MODE");
-      return z != nullptr && std::string(z) == "tma";
-    }();
-    if (!tma_host) {
-      static const int host_ctas = []() {
-        const char* z = std::getenv("B200KV_PACK_HOST_CTAS");
-        return z ? std::max(1, std::atoi(z)) : 96;
-      }();
-      const int grid = n_items < host_ctas ? n_items : host_ctas;
-      pack_ldst_kernel<<<grid, kLdstThreads, 0, stream>>>(d_items, n_items);
-      KV_CUDA(cudaGetLastError());
-      return;
-    }
+  if (host_io) {
+    constexpr int kHostCtas = 96;
+    const int grid = n_items < kHostCtas ? n_items : kHostCtas;
+    pack_ldst_kernel<<<grid, kLdstThreads, 0, stream>>>(d_items, n_items);
+    KV_CUDA(cudaGetLastError());
+    return;
   }
   const int smem = kStages * kPackTileBytes;
   // per-device attribute: set on every launch (cheap) so multi-GPU processes are covered
   KV_CUDA(cudaFuncSetAttribute(pack_bulk_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
   // 3 CTAs of 64 KB fit an SM; enough CTAs to cover all 132 SMs, each looping over its tiles
-  // (PCIe-bound lists get a small grid: 64 KB in flight per CTA already covers the link's
-  // bandwidth-delay product many times over, and the SMs stay free for the fused kernel that runs
-  // beside the transfer)
-  const int cap = max_ctas > 0 ? max_ctas : kNumSMs * 3;
+  const int cap = kNumSMs * 3;
   const int grid = n_items < cap ? n_items : cap;
   pack_bulk_kernel<<<grid, kPackThreads, smem, stream>>>(d_items, n_items);
   KV_CUDA(cudaGetLastError());

@@ -219,7 +219,7 @@ void KVStore::PushRowSparse(KeyEntry& e, const std::vector<NDArray>& srcs_in) {
     merged = MergeRowSparseGroup(e, srcs[0]);
     total = 0;   // the merge is done: skip the single-process union below
   }
-  if (fused && !dense_key && total > 0 && parts.size() >= 2 && std::getenv("B200KV_RSP_SHARD_OFF") == nullptr) {
+  if (fused && !dense_key && total > 0 && parts.size() >= 2) {
     // sources on several GPUs: every GPU merges and updates its own row range of the table
     if (PushRowSparseSharded(e, srcs, parts, U)) return;
   }
