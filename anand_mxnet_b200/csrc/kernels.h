@@ -126,9 +126,13 @@ struct RspUpdateLaunch {
 };
 void LaunchRspUpdate(const RspUpdateLaunch& p, cudaStream_t stream);
 
+// row_map[r] = position of table row r among the `nnr` ascending ids `gidx`, or -1: a memset of
+// int32[table_rows] to -1, then row_map_scatter_kernel when nnr > 0
+void LaunchRowMap(const int64_t* gidx, int64_t nnr, int64_t table_rows, int32_t* row_map,
+                  cudaStream_t stream);
 // standard (non-lazy) update over ALL `table_rows` rows of a dense weight; rows missing from the
-// row_sparse gradient (gidx / gval / nrows or d_nrows of `p`) use grad = 0. row_map: int32[table_rows]
-void LaunchRspStdUpdate(const RspUpdateLaunch& p, int64_t table_rows, int32_t* row_map,
+// row_sparse gradient (gidx / gval / nrows of `p`) use grad = 0. row_map: LaunchRowMap's
+void LaunchRspStdUpdate(const RspUpdateLaunch& p, int64_t table_rows, const int32_t* row_map,
                         cudaStream_t stream);
 // storage casts: ids of the rows with any non-zero element (ascending) + count; scatter rows
 size_t NonzeroRowsWorkspaceBytes(int64_t rows);
@@ -314,8 +318,15 @@ struct UpdateLaunch {
   // `nnr` rows of `row_len` elements, and gradient row r updates table row gidx[r]
   const int64_t* gidx = nullptr;
   int64_t nnr = 0, row_len = 0;
+  // a row_sparse gradient of a dense float32 weight (LaunchRspGradUpdateOp): g holds the stored rows of
+  // `row_len` elements, row_map[r] is table row r's position among them or -1 (LaunchRowMap), and
+  // all `n` elements are updated, those of absent rows with g = +0.0f
+  const int32_t* row_map = nullptr;
 };
 void LaunchUpdateOp(const UpdateLaunch& L, cudaStream_t stream);
+// the float32 operators but mp_nag with a row_sparse gradient (update_rsp_grad_kernels.cu): every
+// element of the dense weight and states moves, absent rows with g = +0.0f
+void LaunchRspGradUpdateOp(const UpdateLaunch& L, cudaStream_t stream);
 // row_sparse forms of ftrl_update and _sparse_adagrad_update (rowsparse_kernels.cu;
 // FtrlDnsRspDnsKernel, AdagradDnsRspDnsKernel: optimizer_op-inl.h:2186-2219, 2507-2531): float32,
 // one warp per gradient row, the same Step<OP> as the dense kernel. Rows not in gidx stay untouched.

@@ -430,6 +430,15 @@ std::function<void()> KVStore::PullRowSparseGroup(int home, const std::vector<si
 // =================================================================================================
 // standard (non-lazy) updates and storage casts
 // =================================================================================================
+NDArray BuildRowMap(LaneOp& op, const NDArray& g, int64_t rows) {
+  NDArray row_map({rows}, Context::GPU(g.dev()), kInt32);
+  op.Write(row_map);
+  const bool stored = g.storage_initialized();
+  LaunchRowMap(stored ? g.row_ids() : nullptr, stored ? g.nnr() : 0, rows,
+               static_cast<int32_t*>(row_map.data()), op.stream());
+  return row_map;
+}
+
 void RunRspStdUpdate(const NDArray& w, const NDArray& g, const NDArray& s1, const NDArray& s2,
                      RspUpdateLaunch L) {
   KV_CHECK(w.on_gpu() && g.on_gpu() && w.dev() == g.dev()) << "all operands must be on the same GPU";
@@ -442,8 +451,8 @@ void RunRspStdUpdate(const NDArray& w, const NDArray& g, const NDArray& s1, cons
     KV_CHECK_EQ(w.nnr(), rows) << "standard sparse update: the row_sparse weight must hold every row";
   }
   LaneOp op(dev);
-  NDArray row_map({rows}, Context::GPU(dev), kInt32);
-  op.Read(g).Write(w).Write(row_map).Write(s1).Write(s2);
+  op.Read(g).Write(w).Write(s1).Write(s2);
+  const NDArray row_map = BuildRowMap(op, g, rows);
   L.w = static_cast<float*>(w.data());
   L.s1 = s1.is_none() ? nullptr : static_cast<float*>(s1.data());
   L.s2 = s2.is_none() ? nullptr : static_cast<float*>(s2.data());
@@ -452,7 +461,7 @@ void RunRspStdUpdate(const NDArray& w, const NDArray& g, const NDArray& s1, cons
   L.nrows = g.nnr();
   L.d_nrows = nullptr;
   L.row_len = static_cast<int64_t>(w.RowLength());
-  LaunchRspStdUpdate(L, rows, static_cast<int32_t*>(row_map.data()), op.stream());
+  LaunchRspStdUpdate(L, rows, static_cast<const int32_t*>(row_map.data()), op.stream());
   Engine::Get()->CountLaunch("rsp_std_update", static_cast<uint64_t>(rows) * L.row_len * 8);
   op.Issue();
 }

@@ -12,6 +12,11 @@ namespace b200kv {
 void RunRspStdUpdate(const NDArray& w, const NDArray& g, const NDArray& s1, const NDArray& s2,
                      RspUpdateLaunch L);
 
+// The row map of a row_sparse gradient `g` over a table of `rows` rows: an int32 per table row, the
+// row's position among g's stored rows or -1 (LaunchRowMap). Declared written by `op` and built on
+// its stream, so it is called after every other operand of `op` is declared.
+NDArray BuildRowMap(LaneOp& op, const NDArray& g, int64_t rows);
+
 // CopyFromTo across storage types (src/ndarray/ndarray.cc:1147-1196 + cast_storage-inl.h:74-140):
 // dense -> row_sparse keeps the rows with a non-zero element, row_sparse -> dense scatters the
 // rows over zeros. float32 only; the cast runs on a GPU (the source's, else the target's).

@@ -693,9 +693,7 @@ __global__ void bm_emit_pull_kernel(const uint32_t* bitmap, const uint32_t* pref
 // rows absent from the gradient see grad = 0 (optimizer_op-inl.h:505-528, optimizer_op.cc:108-139,
 // 195-229). row_map[r] = position of row r in the gradient, or -1.
 
-__global__ void row_map_scatter_kernel(const int64_t* gidx, int64_t nnr_bound, const int64_t* d_nnr,
-                                       int32_t* row_map) {
-  const int64_t nnr = d_nnr ? *d_nnr : nnr_bound;
+__global__ void row_map_scatter_kernel(const int64_t* gidx, int64_t nnr, int32_t* row_map) {
   for (int64_t i = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x; i < nnr;
        i += static_cast<int64_t>(gridDim.x) * blockDim.x) {
     row_map[gidx[i]] = static_cast<int32_t>(i);
@@ -1296,15 +1294,20 @@ void LaunchRetainBatch(int nitems, int64_t total, int id_bits, const int64_t* d_
   KV_CUDA(cudaGetLastError());
 }
 
-void LaunchRspStdUpdate(const RspUpdateLaunch& p, int64_t table_rows, int32_t* row_map,
-                        cudaStream_t stream) {
-  if (table_rows <= 0 || p.row_len <= 0) return;
-  KV_CHECK(p.nrows < (1LL << 31));
+void LaunchRowMap(const int64_t* gidx, int64_t nnr, int64_t table_rows, int32_t* row_map,
+                  cudaStream_t stream) {
+  if (table_rows <= 0) return;
+  KV_CHECK(nnr < (1LL << 31));
   KV_CUDA(cudaMemsetAsync(row_map, 0xff, static_cast<size_t>(table_rows) * sizeof(int32_t), stream));
-  if (p.nrows > 0) {
-    row_map_scatter_kernel<<<GridFor(p.nrows, 256), 256, 0, stream>>>(p.gidx, p.nrows, p.d_nrows, row_map);
+  if (nnr > 0) {
+    row_map_scatter_kernel<<<GridFor(nnr, 256), 256, 0, stream>>>(gidx, nnr, row_map);
     KV_CUDA(cudaGetLastError());
   }
+}
+
+void LaunchRspStdUpdate(const RspUpdateLaunch& p, int64_t table_rows, const int32_t* row_map,
+                        cudaStream_t stream) {
+  if (table_rows <= 0 || p.row_len <= 0) return;
   const int blocks = static_cast<int>((table_rows + kWarpsPerBlock - 1) / kWarpsPerBlock);
   const int threads = kWarpsPerBlock * 32;
   switch (p.opt) {

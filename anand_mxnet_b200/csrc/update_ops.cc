@@ -2,7 +2,9 @@
 // Signum, RMSProp, FTML and Ftrl optimizers call from their `update` (the per-key updater callback
 // of the store, and the local updaters of update_on_kvstore=False), plus the row_sparse forms of
 // ftrl_update, AdaGrad's _sparse_adagrad_update and GroupAdaGrad's _contrib_group_adagrad_update.
-// Kernels: update_kernels.cu (dense), rowsparse_kernels.cu (row_sparse).
+// Kernels: update_kernels.cu and update_rsp_grad_kernels.cu (dense weights, with a dense or a
+// row_sparse gradient), rowsparse_kernels.cu (row_sparse weights, and the lazy dense-weight forms of
+// AdaGrad / GroupAdaGrad).
 //
 // Reference operator definitions (inputs, parameter structs, kernels):
 //   nag_mom_update, mp_nag_mom_update    src/operator/optimizer_op.cc:712-762, optimizer_op-inl.h:1032-1160
@@ -13,10 +15,21 @@
 //   _sparse_adagrad_update               optimizer_op.cc:895-924, optimizer_op-inl.h:2454-2649
 //   _contrib_group_adagrad_update        contrib/optimizer_op.cc:53-86, contrib/optimizer_op-inl.h:46-243
 //
-// Dense float32 arrays (mp_nag_mom_update: float16 / bfloat16 weights with float32 mom and
-// weight32), or the row_sparse forms in float32 (RspUpdateOp). The reference would densify a
-// row_sparse gradient of a dense-weight ftrl_update and run 16-bit weights of the other operators
-// in half precision; both are refused here before anything is launched.
+// Storage forms (UpdateOp), all float32 but mp_nag_mom_update's 16-bit weight and gradient:
+//   all dense                          every operator (mp_nag_mom_update: float16 / bfloat16 weight
+//                                      and gradient with float32 mom and weight32)
+//   dense weight and states, a row_sparse gradient
+//                                      every operator but mp_nag_mom_update. The reference has no
+//                                      FComputeEx for this pair and falls back to the dense
+//                                      FCompute on the densified gradient (imperative_utils.h:
+//                                      185-198, CastStorageRspDnsImpl): every row moves, absent rows
+//                                      with g = +0.0f. Here the kernel reads the stored rows through
+//                                      a row map instead of a dense copy (BuildRowMap).
+//   row_sparse weight, grad and states ftrl_update (RspUpdateOp): only the gradient's rows move
+//   AdaGrad / GroupAdaGrad             their own row_sparse forms (RspUpdateOp)
+// Everything else is refused before anything is enqueued: a row_sparse weight or state with the
+// other operators (the reference would densify the weight, update it and cast it back), and 16-bit
+// weights without a master copy (the reference would update them in half precision).
 #include <cctype>
 #include <cerrno>
 #include <cmath>
@@ -25,6 +38,7 @@
 #include "kernels.h"
 #include "op_params.h"
 #include "ops.h"
+#include "rowsparse.h"
 
 namespace b200kv {
 namespace {
@@ -35,23 +49,25 @@ struct Spec {
   int nin;                 // weight, grad, states...
   const char* launch_name; // CountLaunch keeps the pointer
   int bytes_per_elem;      // algorithmic traffic of one element (float32 / mp float16)
+  const char* rsp_grad_launch_name;  // the dense-weight pass over a row_sparse gradient
 };
 
 const Spec kSpecs[] = {
-    {"nag_mom_update", kUpdNAG, 3, "update_op(nag_mom_update)", 20},
-    {"mp_nag_mom_update", kUpdMPNAG, 4, "update_op(mp_nag_mom_update)", 20},
-    {"signsgd_update", kUpdSignSGD, 2, "update_op(signsgd_update)", 12},
-    {"signum_update", kUpdSignum, 3, "update_op(signum_update)", 20},
-    {"rmsprop_update", kUpdRMSProp, 3, "update_op(rmsprop_update)", 20},
-    {"rmspropalex_update", kUpdRMSPropAlex, 5, "update_op(rmspropalex_update)", 36},
-    {"ftml_update", kUpdFTML, 5, "update_op(ftml_update)", 36},
-    {"ftrl_update", kUpdFtrl, 4, "update_op(ftrl_update)", 28},
-    // row_sparse only: the alias of ftrl_update (MXNET_ADD_SPARSE_OP_ALIAS, optimizer_op.cc:855)
-    // and AdaGrad's operator (optimizer_op.cc:895-924, optimizer_op-inl.h:2454-2649)
-    {"_sparse_ftrl_update", kUpdFtrl, 4, "update_op(ftrl_update)", 28},
-    {"_sparse_adagrad_update", kUpdAdaGrad, 3, "update_op(_sparse_adagrad_update)", 20},
+    {"nag_mom_update", kUpdNAG, 3, "update_op(nag_mom_update)", 20, "update_op(nag_mom_update, row_sparse grad)"},
+    {"mp_nag_mom_update", kUpdMPNAG, 4, "update_op(mp_nag_mom_update)", 20, nullptr},
+    {"signsgd_update", kUpdSignSGD, 2, "update_op(signsgd_update)", 12, "update_op(signsgd_update, row_sparse grad)"},
+    {"signum_update", kUpdSignum, 3, "update_op(signum_update)", 20, "update_op(signum_update, row_sparse grad)"},
+    {"rmsprop_update", kUpdRMSProp, 3, "update_op(rmsprop_update)", 20, "update_op(rmsprop_update, row_sparse grad)"},
+    {"rmspropalex_update", kUpdRMSPropAlex, 5, "update_op(rmspropalex_update)", 36,
+     "update_op(rmspropalex_update, row_sparse grad)"},
+    {"ftml_update", kUpdFTML, 5, "update_op(ftml_update)", 36, "update_op(ftml_update, row_sparse grad)"},
+    {"ftrl_update", kUpdFtrl, 4, "update_op(ftrl_update)", 28, "update_op(ftrl_update, row_sparse grad)"},
+    // the alias of ftrl_update (MXNET_ADD_SPARSE_OP_ALIAS, optimizer_op.cc:855) and AdaGrad's
+    // operator (optimizer_op.cc:895-924, optimizer_op-inl.h:2454-2649)
+    {"_sparse_ftrl_update", kUpdFtrl, 4, "update_op(ftrl_update)", 28, "update_op(ftrl_update, row_sparse grad)"},
+    {"_sparse_adagrad_update", kUpdAdaGrad, 3, "update_op(_sparse_adagrad_update)", 20, nullptr},
     // GroupAdaGrad's operator: g 4 + w 4+4 per element; the history is one float per row
-    {"_contrib_group_adagrad_update", kUpdGroupAdaGrad, 3, "update_op(_contrib_group_adagrad_update)", 12},
+    {"_contrib_group_adagrad_update", kUpdGroupAdaGrad, 3, "update_op(_contrib_group_adagrad_update)", 12, nullptr},
 };
 
 // dmlc::Parameter set_range(lo, hi) (parameter.h:752-762)
@@ -88,8 +104,7 @@ void RspUpdateOp(const Spec& spec, const std::vector<NDArray>& in, std::vector<N
     L.lamda1 = GetF(p, "lamda1", 0.01f);
     L.beta = GetF(p, "beta", 1.0f);
     KV_CHECK(wst == kRowSparseStorage && g.stype() == kRowSparseStorage)
-        << n << ": the row_sparse form needs row_sparse weight, grad, z and n (a dense weight with a "
-        << "row_sparse gradient is not supported)";
+        << n << ": the row_sparse form needs row_sparse weight, grad, z and n";
   } else if (op == kUpdGroupAdaGrad) {  // GroupAdagradParam (contrib/optimizer_op-inl.h:46-65)
     RejectUnknownKeys(p, {"lr", "rescale_grad", "clip_gradient", "epsilon"});  // wd among the unknown
     L.eps = GetF(p, "epsilon", 1.0e-5f);
@@ -163,8 +178,14 @@ void RspUpdateOp(const Spec& spec, const std::vector<NDArray>& in, std::vector<N
   lop.Issue();
 }
 
-// every operator of kSpecs (variant: its index there): the row_sparse forms in RspUpdateOp, the
-// dense ones here
+std::string Stypes(const std::vector<NDArray>& in) {
+  std::string t;
+  for (const NDArray& a : in) t += std::string(t.empty() ? "" : ", ") + StypeName(a.stype());
+  return t;
+}
+
+// every operator of kSpecs (variant: its index there): the row_sparse-weight forms and AdaGrad /
+// GroupAdaGrad in RspUpdateOp, dense weights and states here, with a dense or a row_sparse gradient
 void UpdateOp(const OpInfo& info, const std::vector<NDArray>& in, std::vector<NDArray>* outputs,
               const Params& p) {
   const Spec& spec = kSpecs[info.variant];
@@ -180,14 +201,20 @@ void UpdateOp(const OpInfo& info, const std::vector<NDArray>& in, std::vector<ND
           << in[i].stype() << " and weight.stype = " << w.stype();
     }
   }
-  if (op == kUpdAdaGrad || op == kUpdGroupAdaGrad || w.stype() == kRowSparseStorage) {
+  if (op == kUpdAdaGrad || op == kUpdGroupAdaGrad || (op == kUpdFtrl && w.stype() == kRowSparseStorage)) {
     RspUpdateOp(spec, in, outputs, p);
     return;
   }
-  for (const NDArray& a : in) {
-    KV_CHECK(a.stype() == kDefaultStorage)
-        << n << ": row_sparse weights, gradients or states are not supported (dense arrays only)";
-  }
+  bool dense_tables = w.stype() == kDefaultStorage;
+  for (int i = 2; i < spec.nin; ++i) dense_tables = dense_tables && in[i].stype() == kDefaultStorage;
+  const bool rsp_grad = g.stype() == kRowSparseStorage;
+  KV_CHECK(dense_tables && (rsp_grad || g.stype() == kDefaultStorage))
+      << "Operator " << n << " is not implemented for storage types (" << Stypes(in) << "): it takes a "
+      << "dense weight and dense states with a dense or row_sparse gradient"
+      << (op == kUpdFtrl ? ", or row_sparse weight, grad, z and n" : "");
+  KV_CHECK(!rsp_grad || op != kUpdMPNAG)
+      << n << ": a row_sparse gradient is not supported (16-bit weights would need 16-bit row_sparse "
+      << "values; use nag_mom_update on float32 weights)";
   KV_CHECK(w.on_gpu()) << n << " runs on GPU arrays only (no CPU fallback)";
   const int dev = w.dev();
   const int dtype = w.dtype();
@@ -202,17 +229,25 @@ void UpdateOp(const OpInfo& info, const std::vector<NDArray>& in, std::vector<ND
   for (const NDArray& a : in) {
     KV_CHECK(a.on_gpu() && a.dev() == dev) << n << ": all operands must be on the same GPU";
   }
+  if (rsp_grad) {
+    // ElemwiseShape: every operand has the weight's shape, not only its size
+    KV_CHECK_EQ(g.dtype(), kFloat32) << n << ": row_sparse gradients are float32, got " << DTypeName(g.dtype());
+    KV_CHECK(!w.shape().empty()) << n << ": the weight needs at least one dimension";
+    KV_CHECK(g.shape() == w.shape()) << n << ": weight / grad shape mismatch";
+  }
   KV_CHECK_EQ(g.dtype(), dtype) << n << ": weight / grad dtype mismatch";
   KV_CHECK_EQ(g.Size(), w.Size()) << n << ": weight / grad shape mismatch";
   for (int i = 2; i < spec.nin; ++i) {
     KV_CHECK_EQ(in[i].dtype(), kFloat32) << n << ": optimizer states must be float32";
     KV_CHECK_EQ(in[i].Size(), w.Size()) << n << ": state shape mismatch";
+    KV_CHECK(!rsp_grad || in[i].shape() == w.shape()) << n << ": state shape mismatch";
   }
   NDArray out = OutOr(outputs, 0, w.shape(), w.ctx(), dtype);
   KV_CHECK(out.on_gpu() && out.dev() == dev) << n << ": out must be on the weight's GPU";
   KV_CHECK(out.stype() == kDefaultStorage) << n << ": out must be a dense array";
   KV_CHECK_EQ(out.dtype(), dtype) << n << ": out dtype mismatch";
   KV_CHECK_EQ(out.Size(), w.Size()) << n << ": out shape mismatch";
+  KV_CHECK(!rsp_grad || out.shape() == w.shape()) << n << ": out shape mismatch";
   const bool out_is_w = out.SameStorage(w);
   KV_CHECK(!out_is_w || out.data() == w.data()) << n << ": out overlaps the weight without being it";
 
@@ -269,8 +304,28 @@ void UpdateOp(const OpInfo& info, const std::vector<NDArray>& in, std::vector<ND
   if (!out_is_w) lop.Read(w);
   lop.Write(out);
   for (int i = 2; i < spec.nin; ++i) lop.Write(in[i]);
-  LaunchUpdateOp(L, lop.stream());
-  Engine::Get()->CountLaunch(spec.launch_name, static_cast<uint64_t>(spec.bytes_per_elem) * L.n);
+  if (!rsp_grad) {
+    LaunchUpdateOp(L, lop.stream());
+    Engine::Get()->CountLaunch(spec.launch_name, static_cast<uint64_t>(spec.bytes_per_elem) * L.n);
+    lop.Issue();
+    return;
+  }
+  // the stored rows through a row map, every element of the table updated; an empty gradient is
+  // a full update with g = +0.0f
+  const int64_t rows = w.shape()[0];
+  const NDArray row_map = BuildRowMap(lop, g, rows);
+  L.g = g.storage_initialized() ? g.data() : nullptr;
+  L.nnr = g.nnr();
+  L.row_len = static_cast<int64_t>(w.RowLength());
+  L.row_map = static_cast<const int32_t*>(row_map.data());
+  LaunchRspGradUpdateOp(L, lop.stream());
+  // bytes: the scatter reads an 8 B id and writes 4 B per stored row; the update moves the dense
+  // pass's bytes less the gradient's 4 B per element, reads the stored rows once, and counts the
+  // row map's memset and read (4 B each per table row)
+  if (L.nnr > 0) Engine::Get()->CountLaunch("update_op(row_map_scatter)", static_cast<uint64_t>(L.nnr) * 12);
+  Engine::Get()->CountLaunch(spec.rsp_grad_launch_name,
+                             static_cast<uint64_t>(spec.bytes_per_elem - 4) * L.n +
+                                 static_cast<uint64_t>(L.nnr) * L.row_len * 4 + static_cast<uint64_t>(rows) * 8);
   lop.Issue();
 }
 
