@@ -113,27 +113,20 @@ void LaunchRowMean(int dtype, void* out, const void* in, int64_t rows, int64_t c
 void LaunchCast(void* out, int out_dtype, const void* in, int in_dtype, size_t n, cudaStream_t stream);
 
 // ---- row_sparse (rowsparse_kernels.cu) ----
-// lazy row updates over the rows listed in a row_sparse gradient (optimizer_op-inl.h:426-450,
-// 776-801, 1383-1408); opt is kOptSGDSingle (sgd_update), kOptSGD (sgd_mom_update), kOptAdam
+// the lazy optimizer step that LaunchRspMerge fuses into its row sum (optimizer_op-inl.h:426-450,
+// 776-801, 1383-1408): row `id` of the table w (+ states) takes the summed gradient row; opt is
+// kOptSGDSingle (sgd_update), kOptSGD (sgd_mom_update) or kOptAdam
 struct RspUpdateLaunch {
   float* w = nullptr; float* s1 = nullptr; float* s2 = nullptr;
-  const int64_t* gidx = nullptr; const float* gval = nullptr;
-  int64_t nrows = 0, row_len = 0;
-  const int64_t* d_nrows = nullptr;  // when set: the row count lives on the device, nrows bounds it
   int opt = kOptSGDSingle;
   float lr = 0.f, wd = 0.f, momentum = 0.f, rescale = 1.f, clip = -1.f, beta1 = 0.9f,
         beta2 = 0.999f, eps = 1e-8f;
 };
-void LaunchRspUpdate(const RspUpdateLaunch& p, cudaStream_t stream);
 
 // row_map[r] = position of table row r among the `nnr` ascending ids `gidx`, or -1: a memset of
 // int32[table_rows] to -1, then row_map_scatter_kernel when nnr > 0
 void LaunchRowMap(const int64_t* gidx, int64_t nnr, int64_t table_rows, int32_t* row_map,
                   cudaStream_t stream);
-// standard (non-lazy) update over ALL `table_rows` rows of a dense weight; rows missing from the
-// row_sparse gradient (gidx / gval / nrows of `p`) use grad = 0. row_map: LaunchRowMap's
-void LaunchRspStdUpdate(const RspUpdateLaunch& p, int64_t table_rows, const int32_t* row_map,
-                        cudaStream_t stream);
 // storage casts: ids of the rows with any non-zero element (ascending) + count; scatter rows
 size_t NonzeroRowsWorkspaceBytes(int64_t rows);
 void LaunchNonzeroRows(const float* data, int64_t rows, int64_t row_len, int64_t* out_idx,
@@ -297,9 +290,12 @@ int LaunchResetArrays(ResetArraysList& arrays, cudaStream_t stream);
 
 // ---- single-tensor optimizer operators of the callback route (update_kernels.cu) ----
 // nag_mom_update, mp_nag_mom_update, signsgd_update, signum_update, rmsprop_update,
-// rmspropalex_update, ftml_update, ftrl_update (optimizer_op-inl.h:1061-1222, 1953-2158, 2344-2431)
+// rmspropalex_update, ftml_update, ftrl_update (optimizer_op-inl.h:1061-1222, 1953-2158, 2344-2431).
+// The row_sparse-gradient forms of sgd_update, sgd_mom_update and adam_update: kUpdSGD, kUpdAdamLazy
+// lazy (only the gradient's rows), kUpdSGDStd, kUpdAdamStd standard (every row), kUpdSGDMom both.
 enum UpdOp : int { kUpdNAG = 0, kUpdMPNAG, kUpdSignSGD, kUpdSignum, kUpdRMSProp, kUpdRMSPropAlex,
-                   kUpdFTML, kUpdFtrl, kUpdAdaGrad, kUpdGroupAdaGrad };
+                   kUpdFTML, kUpdFtrl, kUpdAdaGrad, kUpdGroupAdaGrad,
+                   kUpdSGD, kUpdSGDStd, kUpdSGDMom, kUpdAdamLazy, kUpdAdamStd };
 struct UpdateLaunch {
   int op = kUpdNAG;
   int dtype = 0;                 // of w / g / out: kFloat32, or kFloat16 / kBfloat16 for kUpdMPNAG
@@ -325,10 +321,12 @@ struct UpdateLaunch {
 };
 void LaunchUpdateOp(const UpdateLaunch& L, cudaStream_t stream);
 // the float32 operators but mp_nag with a row_sparse gradient (update_rsp_grad_kernels.cu): every
-// element of the dense weight and states moves, absent rows with g = +0.0f
+// element of the dense weight and states moves, absent rows with g = +0.0f; also the standard forms
+// of sgd_update, sgd_mom_update and adam_update (kUpdSGDStd, kUpdSGDMom, kUpdAdamStd)
 void LaunchRspGradUpdateOp(const UpdateLaunch& L, cudaStream_t stream);
 // row_sparse forms of ftrl_update and _sparse_adagrad_update (rowsparse_kernels.cu;
-// FtrlDnsRspDnsKernel, AdagradDnsRspDnsKernel: optimizer_op-inl.h:2186-2219, 2507-2531): float32,
+// FtrlDnsRspDnsKernel, AdagradDnsRspDnsKernel: optimizer_op-inl.h:2186-2219, 2507-2531) and the lazy
+// forms of sgd_update, sgd_mom_update and adam_update (kUpdSGD, kUpdSGDMom, kUpdAdamLazy): float32,
 // one warp per gradient row, the same Step<OP> as the dense kernel. Rows not in gidx stay untouched.
 // kUpdGroupAdaGrad (_contrib_group_adagrad_update, GroupAdagradDnsRspKernel: contrib/
 // optimizer_op-inl.h:96-139): s[0] is the history, one float per table row; each row's sum of

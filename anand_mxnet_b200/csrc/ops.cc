@@ -68,6 +68,24 @@ void ZeroFillEmptyRspStates(const std::vector<NDArray>& states, int64_t rows, co
   lop.Issue();
 }
 
+void CheckRspTable(const char* op, const char* func, const std::vector<NDArray>& in,
+                   const std::vector<NDArray>& outputs) {
+  const NDArray& w = in[0];
+  const int64_t rows = w.shape()[0];
+  KV_CHECK(w.stype() != kRowSparseStorage || w.nnr() == rows)
+      << func << " for RowSparse weights is only implemented for RowSparse weights with all rows "
+      << "containing non-zeros. Expects weights.data.shape[0] (" << w.nnr() << ") == weights.shape[0] ("
+      << rows << ").";
+  for (size_t i = 2; i < in.size(); ++i) {
+    KV_CHECK(in[i].stype() != kRowSparseStorage || in[i].nnr() == 0 || in[i].nnr() == rows)
+        << op << ": a row_sparse optimizer state must hold every row or none (it holds "
+        << in[i].nnr() << " of " << rows << ")";
+  }
+  KV_CHECK(outputs.size() == 1 && outputs[0].SameStorage(w) && outputs[0].stype() == w.stype() &&
+           outputs[0].data() == w.data())
+      << op << ": out must be the weight itself (kWriteInplace is expected for sparse " << op << ")";
+}
+
 const OpInfo* FindOp(const std::string& name) {
   static const auto* table = [] {
     auto* m = new std::unordered_map<std::string, const OpInfo*>();
@@ -240,29 +258,6 @@ void RunAdhoc(int opt, std::vector<AdhocKey>& keys, const DenseLaunch& scalars,
   op.Issue();
 }
 
-// lazy row_sparse gradient: update only the rows listed (optimizer_op-inl.h:452-565,803-876,1410-1470).
-// w is dense, or row_sparse with every row (SgdAdamRspWeight has checked it): either way its values
-// are the row-major table, addressed by the gradient's row ids.
-void RunRspUpdate(int opt, const NDArray& w, const NDArray& g, const NDArray& s1, const NDArray& s2,
-                  RspUpdateLaunch L) {
-  KV_CHECK(w.on_gpu() && g.on_gpu() && w.dev() == g.dev()) << "all operands must be on the same GPU";
-  KV_CHECK_EQ(w.dtype(), kFloat32) << "row_sparse optimizer updates are float32";
-  if (!g.storage_initialized()) return;  // all-zero gradient: lazy update touches nothing
-  LaneOp op(w.dev());
-  op.Read(g).Write(w).Write(s1).Write(s2);
-  L.opt = opt;
-  L.w = static_cast<float*>(w.data());
-  L.s1 = s1.is_none() ? nullptr : static_cast<float*>(s1.data());
-  L.s2 = s2.is_none() ? nullptr : static_cast<float*>(s2.data());
-  L.gidx = g.row_ids();
-  L.gval = static_cast<const float*>(g.data());
-  L.nrows = g.nnr();
-  L.row_len = static_cast<int64_t>(w.RowLength());
-  LaunchRspUpdate(L, op.stream());
-  Engine::Get()->CountLaunch("rsp_update", 0);
-  op.Issue();
-}
-
 // Weight dtypes, checked before InPlace copies a weight into a distinct out. The fused step computes
 // in float32 and rounds once on store. The reference's non-mp forms compute in the weight's own
 // type and round after every operation (optimizer_op-inl.h:225-250, 410-418), so they take float32
@@ -301,47 +296,26 @@ DenseLaunch GradScalars(const Params& p) {
 // serve it. A row_sparse state holds every row, or none yet: then it is zero-filled first, in both
 // forms and even when the gradient is empty. Every check runs before anything is enqueued.
 void SgdAdamRspWeight(const OpInfo& op, const std::vector<NDArray>& in, std::vector<NDArray>* outputs,
-                      RspUpdateLaunch L, bool lazy) {
+                      const UpdateLaunch& L, bool lazy) {
   const NDArray& w = in[0];
-  const NDArray& g = in[1];
   const int kind = op.variant;
   if (in.size() > 2 && in[2].stype() == kDefaultStorage) lazy = false;  // StdOptStorageType (:912-917)
   KV_CHECK(!w.shape().empty()) << op.name << ": the weight needs at least one dimension";
-  const int64_t rows = w.shape()[0];
   for (const NDArray& a : in) {
     KV_CHECK(a.on_gpu() && a.dev() == w.dev()) << op.name << ": all operands must be on the same GPU";
     KV_CHECK_EQ(a.dtype(), kFloat32) << "row_sparse optimizer updates are float32";
     KV_CHECK(a.shape() == w.shape()) << op.name << ": weight / grad / state shape mismatch";
   }
-  // CheckAllRowsPresent (operator_common.h:500-511) under the reference's function names
-  // (optimizer_op-inl.h:541, 859, 958, 1472, 1523)
+  // the reference's function names (optimizer_op-inl.h:541, 859, 958, 1472, 1523); kWriteInplace is
+  // expected (optimizer_op-inl.h:497, 818, 1426)
   const char* func = kind == kOptSGDSingle ? "SGDUpdate"
                      : kind == kOptSGD     ? "SGDMomUpdate"
                      : lazy                ? "AdamUpdate"
                                            : "AdamStdUpdate";
-  KV_CHECK(w.nnr() == rows)
-      << func << " for RowSparse weights is only implemented for RowSparse weights with all rows "
-      << "containing non-zeros. Expects weights.data.shape[0] (" << w.nnr() << ") == weights.shape[0] ("
-      << rows << ").";
-  for (size_t i = 2; i < in.size(); ++i) {
-    KV_CHECK(in[i].stype() != kRowSparseStorage || in[i].nnr() == 0 || in[i].nnr() == rows)
-        << op.name << ": a row_sparse optimizer state must hold every row or none (it holds "
-        << in[i].nnr() << " of " << rows << ")";
-  }
-  // kWriteInplace is expected (optimizer_op-inl.h:497, 818, 1426)
-  KV_CHECK(outputs->size() == 1 && (*outputs)[0].SameStorage(w) && (*outputs)[0].data() == w.data())
-      << op.name << ": out must be the weight itself (kWriteInplace is expected for sparse " << op.name
-      << ")";
+  CheckRspTable(op.name, func, in, *outputs);
   const std::vector<NDArray> states(in.begin() + 2, in.end());
-  ZeroFillEmptyRspStates(states, rows, "rsp_state_fill");
-  const NDArray s1 = states.size() > 0 ? states[0] : NDArray();
-  const NDArray s2 = states.size() > 1 ? states[1] : NDArray();
-  L.opt = kind;
-  if (lazy) {
-    RunRspUpdate(kind, w, g, s1, s2, L);
-  } else {
-    RunRspStdUpdate(w, g, s1, s2, L);
-  }
+  ZeroFillEmptyRspStates(states, w.shape()[0], "rsp_state_fill");
+  SgdAdamRspUpdate(kind, lazy, L, w, in[1], states);
 }
 
 // sgd_update, sgd_mom_update, adam_update (variant: the kOpt* kernel code): dense weight with a dense
@@ -371,7 +345,7 @@ void SgdAdam(const OpInfo& op, const std::vector<NDArray>& in, std::vector<NDArr
         << "row_sparse weight, and a row_sparse weight a row_sparse gradient";
   }
   auto rsp_launch = [&] {
-    RspUpdateLaunch L;
+    UpdateLaunch L;
     L.lr = GetF(p, "lr", 0.f);
     L.wd = GetF(p, "wd", 0.f);
     L.momentum = GetF(p, "momentum", 0.f);
@@ -389,15 +363,10 @@ void SgdAdam(const OpInfo& op, const std::vector<NDArray>& in, std::vector<NDArr
   }
   NDArray w = InPlace(in, 0, outputs, 0);
   if (rsp_g) {
-    RspUpdateLaunch L = rsp_launch();
-    if (GetB(p, "lazy_update", true)) {
-      RunRspUpdate(kind, w, in[1], (mom || adam) ? in[2] : NDArray(), adam ? in[3] : NDArray(), L);
-    } else {
-      // standard update: every row moves (SGDUpdateEx / SGDMomUpdateEx / AdamUpdateEx with
-      // lazy_update=False, optimizer_op-inl.h:540-565, 955-1004, 1520-1564)
-      L.opt = kind;
-      RunRspStdUpdate(w, in[1], (mom || adam) ? in[2] : NDArray(), adam ? in[3] : NDArray(), L);
-    }
+    // SGDUpdateEx / SGDMomUpdateEx / AdamUpdateEx (optimizer_op-inl.h:540-565, 955-1004, 1520-1564)
+    const UpdateLaunch L = rsp_launch();
+    SgdAdamRspUpdate(kind, GetB(p, "lazy_update", true), L, w, in[1],
+                     std::vector<NDArray>(in.begin() + 2, in.end()));
     return;
   }
   AdhocKey k;

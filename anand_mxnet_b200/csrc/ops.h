@@ -55,6 +55,13 @@ const char* StypeName(int stype);
 // arrays that hold rows are left alone. launch_name is kept by Engine::CountLaunch.
 void ZeroFillEmptyRspStates(const std::vector<NDArray>& states, int64_t rows, const char* launch_name);
 
+// The operands of a row_sparse optimizer operator `op` whose rows are addressed by table row id:
+// in[0] the weight, in[2...] the states. A row_sparse weight holds every row (CheckAllRowsPresent,
+// operator_common.h:500-511, under the reference's function name `func`), a row_sparse state holds
+// every row or none, and the one out is the weight itself (kWriteInplace).
+void CheckRspTable(const char* op, const char* func, const std::vector<NDArray>& in,
+                   const std::vector<NDArray>& outputs);
+
 // out = op(a[, b], scalar[, scalar2]) through LaunchElementwise (an EwOp code) on out's GPU, after
 // checking that every operand is a dense array on that GPU with out's size and dtype. A failed
 // check throws before anything is enqueued.

@@ -74,14 +74,25 @@ __device__ __forceinline__ float step_adam_lazy(float w, float g, float& s1, flo
   return __fsub_rn(w, __fdiv_rn(__fmul_rn(h.lr, s1), __fadd_rn(__fsqrt_rn(s2), h.eps)));
 }
 
+// AdamStdDnsRspDnsKernel<req,cpu> (optimizer_op.cc:195-229): absent rows use g' = w*wd, and the
+// variance squares first -- (1-beta2)*(g'*g') -- with or without clipping
+__device__ __forceinline__ float step_adam_std(float w, float g, bool present, float& s1, float& s2,
+                                               const Hyper& h) {
+  float gr = present ? __fadd_rn(__fmul_rn(g, h.rescale), __fmul_rn(w, h.wd)) : __fmul_rn(w, h.wd);
+  if (h.clip >= 0.f) gr = clipf(gr, h.clip);
+  s1 = __fadd_rn(__fmul_rn(h.beta1, s1), __fmul_rn(__fsub_rn(1.f, h.beta1), gr));
+  s2 = __fadd_rn(__fmul_rn(h.beta2, s2), __fmul_rn(__fsub_rn(1.f, h.beta2), __fmul_rn(gr, gr)));
+  return __fsub_rn(w, __fdiv_rn(__fmul_rn(h.lr, s1), __fadd_rn(__fsqrt_rn(s2), h.eps)));
+}
+
 // ---- the single-tensor operators of the callback route: the dense elementwise kernel
 // (update_kernels.cu) and the row-gather kernel of their row_sparse forms (rowsparse_kernels.cu)
 
 // fp32 state arrays of each operator (input order after weight, grad) and whether it reads weight
 __host__ __device__ constexpr int NumStates(int op) {
-  return op == kUpdSignSGD ? 0
-         : (op == kUpdNAG || op == kUpdSignum || op == kUpdRMSProp || op == kUpdAdaGrad) ? 1
-         : (op == kUpdMPNAG || op == kUpdFtrl) ? 2 : 3;
+  return (op == kUpdSignSGD || op == kUpdSGD || op == kUpdSGDStd) ? 0
+         : (op == kUpdNAG || op == kUpdSignum || op == kUpdRMSProp || op == kUpdAdaGrad || op == kUpdSGDMom) ? 1
+         : (op == kUpdMPNAG || op == kUpdFtrl || op == kUpdAdamLazy || op == kUpdAdamStd) ? 2 : 3;
 }
 __host__ __device__ constexpr bool ReadsWeight(int op) { return op != kUpdMPNAG; }
 
@@ -89,9 +100,24 @@ __host__ __device__ constexpr bool ReadsWeight(int op) { return op != kUpdMPNAG;
 __device__ __forceinline__ float SignInt(float x) { return static_cast<float>((x > 0.f) - (x < 0.f)); }
 
 // One element. w: weight (unused by mp_nag), g: gradient, s: the states, updated in place.
-// Returns the value stored to out.
+// present: the element's row is stored in a row_sparse gradient (g is +0.0f when it is not); only
+// the standard sgd_update / adam_update forms tell the two apart. Returns the value stored to out.
 template <int OP>
-__device__ __forceinline__ float Step(const UpdateLaunch& a, float w, float g, float (&s)[3]) {
+__device__ __forceinline__ float Step(const UpdateLaunch& a, float w, float g, float (&s)[3],
+                                      bool present = true) {
+  if (OP == kUpdSGD || OP == kUpdSGDStd || OP == kUpdSGDMom || OP == kUpdAdamLazy || OP == kUpdAdamStd) {
+    const Hyper h{a.lr, a.wd, a.momentum, a.rescale, a.clip, a.beta1, a.beta2, a.eps};
+    if (OP == kUpdSGD) return step<kOptSGDSingle>(w, g, s[0], s[1], false, h);
+    if (OP == kUpdSGDMom) return step<kOptSGD>(w, g, s[0], s[1], true, h);  // g = +0.0f when absent
+    if (OP == kUpdAdamLazy) return step_adam_lazy(w, g, s[0], s[1], h);
+    if (OP == kUpdAdamStd) return step_adam_std(w, g, present, s[0], s[1], h);
+    // standard sgd_update: the whole weight is scaled by (1 - lr*wd); present rows then take the
+    // SGDDnsRspKernel step with wd = 0, i.e. (1.f - lr*0.f)*w' - ... = w' - ...
+    const float scaled = __fmul_rn(w, __fsub_rn(1.f, __fmul_rn(h.lr, h.wd)));
+    if (!present) return scaled;
+    if (h.clip >= 0.f) return __fsub_rn(scaled, __fmul_rn(h.lr, clipf(__fmul_rn(h.rescale, g), h.clip)));
+    return __fsub_rn(scaled, __fmul_rn(__fmul_rn(h.lr, h.rescale), g));
+  }
   if (OP == kUpdNAG || OP == kUpdMPNAG) {
     // NAGMomKernel / MP_NAGMomKernel (optimizer_op-inl.h:1061-1138): mom = momentum*mom first;
     // out = (w - mom) + (momentum+1)*(mom - lr*(clip(rescale*g) + wd*w)); then

@@ -163,7 +163,7 @@ void KVStore::PushRowSparse(KeyEntry& e, const std::vector<NDArray>& srcs_in) {
   const int64_t row_len = static_cast<int64_t>(W.RowLength());
   const bool on_store = opt_.enabled && (opt_.kind == kOptSGD || opt_.kind == kOptAdam);
   // lazy: the optimizer step is fused into the row-sum kernel. standard (lazy_update=False): the
-  // merged gradient is materialised, then every row of the table is updated (RunRspStdUpdate).
+  // merged gradient is materialised, then every row of the table is updated (SgdAdamRspUpdate).
   const bool fused = on_store && opt_.lazy_update;
   RspUpdateLaunch U;
   if (on_store) {
@@ -206,7 +206,6 @@ void KVStore::PushRowSparse(KeyEntry& e, const std::vector<NDArray>& srcs_in) {
     U.w = sharded_now ? nullptr : static_cast<float*>(W.data());
     U.s1 = s.s1.is_none() ? nullptr : static_cast<float*>(s.s1.data());
     U.s2 = s.s2.is_none() ? nullptr : static_cast<float*>(s.s2.data());
-    U.row_len = row_len;
   }
   if (dist_) {
     KV_CHECK(!nccl_) << "kvstore 'nccl' handles dense keys only, as the reference's does "
@@ -263,7 +262,16 @@ void KVStore::PushRowSparse(KeyEntry& e, const std::vector<NDArray>& srcs_in) {
   if (fused) return;
   if (on_store) {
     DevState& ds = e.dev[home];
-    RunRspStdUpdate(W, merged, ds.s1, ds.s2, U);
+    UpdateLaunch L;
+    L.lr = U.lr;
+    L.wd = U.wd;
+    L.momentum = U.momentum;
+    L.rescale = U.rescale;
+    L.clip = U.clip;
+    L.beta1 = U.beta1;
+    L.beta2 = U.beta2;
+    L.eps = U.eps;
+    SgdAdamRspUpdate(U.opt, false, L, W, merged, {ds.s1, ds.s2});
     return;
   }
   if (callback) {
@@ -439,31 +447,96 @@ NDArray BuildRowMap(LaneOp& op, const NDArray& g, int64_t rows) {
   return row_map;
 }
 
-void RunRspStdUpdate(const NDArray& w, const NDArray& g, const NDArray& s1, const NDArray& s2,
-                     RspUpdateLaunch L) {
+namespace {
+
+void SetStates(UpdateLaunch& L, const std::vector<NDArray>& states) {
+  KV_CHECK(states.size() <= 3) << "an optimizer step takes at most three states";
+  for (size_t i = 0; i < states.size(); ++i) {
+    L.s[i] = states[i].is_none() ? nullptr : static_cast<float*>(states[i].data());
+  }
+}
+
+}  // namespace
+
+void RunRspRowUpdate(UpdateLaunch L, const NDArray& w, const NDArray& g, const std::vector<NDArray>& states,
+                     const char* launch_name, int bytes_per_elem) {
+  KV_CHECK(w.on_gpu() && g.on_gpu() && w.dev() == g.dev()) << "all operands must be on the same GPU";
+  KV_CHECK_EQ(w.dtype(), kFloat32) << "row_sparse optimizer updates are float32";
+  if (!g.storage_initialized()) return;  // an all-zero gradient changes nothing
+  LaneOp op(w.dev());
+  op.Read(g).Write(w);
+  for (const NDArray& s : states) op.Write(s);
+  L.dtype = kFloat32;
+  L.w = w.data();
+  L.out = w.data();
+  L.g = g.data();
+  L.gidx = g.row_ids();
+  L.nnr = g.nnr();
+  L.row_len = static_cast<int64_t>(w.RowLength());
+  SetStates(L, states);
+  LaunchRspRowUpdateOp(L, op.stream());
+  // + 8 B of id per row, and GroupAdaGrad's history value read and written
+  const int64_t per_row = L.op == kUpdGroupAdaGrad ? 16 : 8;
+  Engine::Get()->CountLaunch(launch_name, static_cast<uint64_t>(L.nnr) * (bytes_per_elem * L.row_len + per_row));
+  op.Issue();
+}
+
+void RunRspGradUpdate(UpdateLaunch L, const NDArray& w, const NDArray& g, const std::vector<NDArray>& states,
+                      const NDArray& out, const char* launch_name, int bytes_per_elem) {
   KV_CHECK(w.on_gpu() && g.on_gpu() && w.dev() == g.dev()) << "all operands must be on the same GPU";
   KV_CHECK_EQ(w.dtype(), kFloat32) << "row_sparse optimizer updates are float32";
   KV_CHECK_EQ(g.stype(), kRowSparseStorage);
-  const int dev = w.dev();
   const int64_t rows = w.shape()[0];
   if (w.stype() == kRowSparseStorage) {
     // CheckAllRowsPresent (optimizer_op-inl.h:532-536)
     KV_CHECK_EQ(w.nnr(), rows) << "standard sparse update: the row_sparse weight must hold every row";
   }
-  LaneOp op(dev);
-  op.Read(g).Write(w).Write(s1).Write(s2);
+  const bool out_is_w = out.SameStorage(w);
+  LaneOp op(w.dev());
+  op.Read(g);
+  if (!out_is_w) op.Read(w);
+  op.Write(out);
+  for (const NDArray& s : states) op.Write(s);
+  // the stored rows through a row map, every element of the table updated; an empty gradient is
+  // a full update with g = +0.0f
   const NDArray row_map = BuildRowMap(op, g, rows);
-  L.w = static_cast<float*>(w.data());
-  L.s1 = s1.is_none() ? nullptr : static_cast<float*>(s1.data());
-  L.s2 = s2.is_none() ? nullptr : static_cast<float*>(s2.data());
-  L.gidx = g.storage_initialized() ? g.row_ids() : nullptr;
-  L.gval = g.storage_initialized() ? static_cast<const float*>(g.data()) : nullptr;
-  L.nrows = g.nnr();
-  L.d_nrows = nullptr;
+  L.dtype = kFloat32;
+  L.w = w.data();
+  L.out = out.data();
+  L.out_is_w = out_is_w;
+  L.n = w.Size();
+  L.g = g.storage_initialized() ? g.data() : nullptr;
+  L.nnr = g.nnr();
   L.row_len = static_cast<int64_t>(w.RowLength());
-  LaunchRspStdUpdate(L, rows, static_cast<const int32_t*>(row_map.data()), op.stream());
-  Engine::Get()->CountLaunch("rsp_std_update", static_cast<uint64_t>(rows) * L.row_len * 8);
+  L.row_map = static_cast<const int32_t*>(row_map.data());
+  SetStates(L, states);
+  LaunchRspGradUpdateOp(L, op.stream());
+  // bytes: the scatter reads an 8 B id and writes 4 B per stored row; the update moves the dense
+  // pass's bytes less the gradient's 4 B per element, reads the stored rows once, and counts the
+  // row map's memset and read (4 B each per table row)
+  if (L.nnr > 0) Engine::Get()->CountLaunch("update_op(row_map_scatter)", static_cast<uint64_t>(L.nnr) * 12);
+  Engine::Get()->CountLaunch(launch_name, static_cast<uint64_t>(bytes_per_elem - 4) * L.n +
+                                              static_cast<uint64_t>(L.nnr) * L.row_len * 4 +
+                                              static_cast<uint64_t>(rows) * 8);
   op.Issue();
+}
+
+void SgdAdamRspUpdate(int kind, bool lazy, UpdateLaunch L, const NDArray& w, const NDArray& g,
+                      const std::vector<NDArray>& states) {
+  // g 4 + w 8, + 8 per state
+  const int bytes = kind == kOptAdam ? 28 : kind == kOptSGD ? 20 : 12;
+  if (kind == kOptSGD) {
+    L.op = kUpdSGDMom;
+  } else if (kind == kOptAdam) {
+    L.op = lazy ? kUpdAdamLazy : kUpdAdamStd;
+  } else {
+    L.op = lazy ? kUpdSGD : kUpdSGDStd;
+  }
+  if (lazy) {
+    RunRspRowUpdate(L, w, g, states, "rsp_update", bytes);
+  } else {
+    RunRspGradUpdate(L, w, g, states, w, "rsp_std_update", bytes);
+  }
 }
 
 void CastStorageCopy(const NDArray& from_in, const NDArray& to) {
@@ -893,7 +966,6 @@ void KVStore::PushRowSparseGroup(KeyEntry& e, const NDArray& src_in, RspUpdateLa
   GroupBarrier();
   if (run) {
     RspUpdateLaunch Uj = U;
-    Uj.row_len = row_len;
     Uj.w = static_cast<float*>(e.rsp_shards[0].data()) - lo * row_len;
     Uj.s1 = need1 ? static_cast<float*>(st8.s1.data()) - lo * row_len : nullptr;
     Uj.s2 = need2 ? static_cast<float*>(st8.s2.data()) - lo * row_len : nullptr;

@@ -1,16 +1,33 @@
 // rowsparse.h -- row_sparse helpers shared by the store (rowsparse.cc), the imperative operators
 // (ops.cc) and CopyFromTo (ndarray.cc).
 #pragma once
+#include <vector>
+
 #include "kernels.h"
 #include "ndarray.h"
 
 namespace b200kv {
 
-// Standard (non-lazy) optimizer step with a row_sparse gradient: every row of the dense weight
-// `w` (and of the dense states) moves; rows absent from `g` see grad = 0
-// (optimizer_op-inl.h:505-528, optimizer_op.cc:108-139, 195-229). `L` carries opt + scalars.
-void RunRspStdUpdate(const NDArray& w, const NDArray& g, const NDArray& s1, const NDArray& s2,
-                     RspUpdateLaunch L);
+// An optimizer step with the row_sparse gradient `g` on a float32 table `w` whose rows are addressed
+// by table row id: w is dense, or row_sparse with every row, and so is each of `states` (in the
+// operator's input order; entries past the op's own states are not read and may be none). `L`
+// carries the op (kUpd*) and its scalars.
+// CountLaunch keeps `launch_name`; bytes_per_elem is the op's algorithmic traffic per element.
+// Lazy: only the rows listed in g move, w in place (LaunchRspRowUpdateOp). An empty g changes nothing.
+void RunRspRowUpdate(UpdateLaunch L, const NDArray& w, const NDArray& g, const std::vector<NDArray>& states,
+                     const char* launch_name, int bytes_per_elem);
+// Standard: every element of the table moves into `out` (w itself, or a dense array of w's shape),
+// rows absent from g with g = +0.0f (LaunchRspGradUpdateOp over the row map of BuildRowMap).
+void RunRspGradUpdate(UpdateLaunch L, const NDArray& w, const NDArray& g, const std::vector<NDArray>& states,
+                      const NDArray& out, const char* launch_name, int bytes_per_elem);
+
+// sgd_update (kind kOptSGDSingle), sgd_mom_update (kOptSGD) or adam_update (kOptAdam) with a
+// row_sparse gradient, in place on w: the lazy form (only g's rows move, optimizer_op-inl.h:426-475,
+// 749-801, 1383-1408) or the standard form (every row, optimizer_op-inl.h:505-528, optimizer_op.cc:
+// 108-139, 195-229). `L` carries the scalars; states starts with mom (sgd_mom_update) or mean and
+// var (adam_update).
+void SgdAdamRspUpdate(int kind, bool lazy, UpdateLaunch L, const NDArray& w, const NDArray& g,
+                      const std::vector<NDArray>& states);
 
 // The row map of a row_sparse gradient `g` over a table of `rows` rows: an int32 per table row, the
 // row's position among g's stored rows or -1 (LaunchRowMap). Declared written by `op` and built on

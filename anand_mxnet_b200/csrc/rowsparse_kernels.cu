@@ -57,61 +57,15 @@ __device__ __forceinline__ int find_segment(const int64_t* start, int nseg, int6
 }
 
 // ---------------------------------------------------------------------------------------------
-template <int OPT>
-__global__ void __launch_bounds__(kWarpsPerBlock * 32) rsp_update_kernel(RspUpdateLaunch p) {
-  const int64_t row = static_cast<int64_t>(blockIdx.x) * kWarpsPerBlock + (threadIdx.x >> 5);
-  const int64_t nrows = p.d_nrows ? *p.d_nrows : p.nrows;
-  if (row >= nrows) return;
-  const int lane = threadIdx.x & 31;
-  Hyper h{p.lr, p.wd, p.momentum, p.rescale, p.clip, p.beta1, p.beta2, p.eps};
-  const int64_t wrow = p.gidx[row];
-  float* w = p.w + wrow * p.row_len;
-  float* s1 = p.s1 ? p.s1 + wrow * p.row_len : nullptr;
-  float* s2 = p.s2 ? p.s2 + wrow * p.row_len : nullptr;
-  const float* g = p.gval + row * p.row_len;
-  const bool vec = (p.row_len % 4 == 0) && ((reinterpret_cast<uintptr_t>(p.w) & 15) == 0) &&
-                   ((reinterpret_cast<uintptr_t>(p.gval) & 15) == 0) &&
-                   (!p.s1 || (reinterpret_cast<uintptr_t>(p.s1) & 15) == 0) &&
-                   (!p.s2 || (reinterpret_cast<uintptr_t>(p.s2) & 15) == 0);
-  auto one = [&](float wv, float gv, float& a, float& b) -> float {
-    if (OPT == kOptAdam) return step_adam_lazy(wv, gv, a, b, h);
-    return step<OPT>(wv, gv, a, b, OPT == kOptSGD, h);
-  };
-  if (vec) {
-    const int64_t nv = p.row_len / 4;
-    for (int64_t v = lane; v < nv; v += 32) {
-      float4 wv = reinterpret_cast<float4*>(w)[v];
-      const float4 gv = __ldcs(reinterpret_cast<const float4*>(g) + v);
-      float4 a = make_float4(0, 0, 0, 0), b = make_float4(0, 0, 0, 0);
-      if (OPT == kOptSGD || OPT == kOptAdam) a = reinterpret_cast<float4*>(s1)[v];
-      if (OPT == kOptAdam) b = reinterpret_cast<float4*>(s2)[v];
-      wv.x = one(wv.x, gv.x, a.x, b.x);
-      wv.y = one(wv.y, gv.y, a.y, b.y);
-      wv.z = one(wv.z, gv.z, a.z, b.z);
-      wv.w = one(wv.w, gv.w, a.w, b.w);
-      reinterpret_cast<float4*>(w)[v] = wv;
-      if (OPT == kOptSGD || OPT == kOptAdam) reinterpret_cast<float4*>(s1)[v] = a;
-      if (OPT == kOptAdam) reinterpret_cast<float4*>(s2)[v] = b;
-    }
-  } else {
-    for (int64_t j = lane; j < p.row_len; j += 32) {
-      float a = 0.f, b = 0.f;
-      if (OPT == kOptSGD || OPT == kOptAdam) a = s1[j];
-      if (OPT == kOptAdam) b = s2[j];
-      w[j] = one(w[j], g[j], a, b);
-      if (OPT == kOptSGD || OPT == kOptAdam) s1[j] = a;
-      if (OPT == kOptAdam) s2[j] = b;
-    }
-  }
-}
-
-// row_sparse forms of the callback route's operators (ftrl_update, _sparse_adagrad_update): one
-// warp per gradient row in a grid-stride loop, the row id read once per row, then the row's
-// elements through the same Step<OP> as the dense update_kernel; out is the weight itself
+// row_sparse forms of the operators (ftrl_update, _sparse_adagrad_update, lazy sgd_update /
+// sgd_mom_update / adam_update): one warp per gradient row in a grid-stride loop, the row id read
+// once per row, then the row's elements through the same Step<OP> as the dense update_kernel; out is
+// the weight itself
 template <int OP>
 __global__ void __launch_bounds__(kWarpsPerBlock * 32) rsp_row_update_kernel(const UpdateLaunch a,
                                                                               const bool vec) {
   constexpr int NS = NumStates(OP);
+  constexpr int NA = NS > 0 ? NS : 1;  // sgd_update has no state, an array needs one entry
   const int lane = threadIdx.x & 31;
   const int64_t nwarps = static_cast<int64_t>(gridDim.x) * kWarpsPerBlock;
   const int64_t len = a.row_len;
@@ -120,18 +74,18 @@ __global__ void __launch_bounds__(kWarpsPerBlock * 32) rsp_row_update_kernel(con
     const int64_t off = a.gidx[r] * len;
     const float* g = static_cast<const float*>(a.g) + r * len;
     float* w = static_cast<float*>(a.out) + off;
-    float* s[NS];
+    float* s[NA];
 #pragma unroll
     for (int k = 0; k < NS; ++k) s[k] = a.s[k] + off;
     if (vec) {
       for (int64_t v = lane; v < len / 4; v += 32) {
         const float4 g4 = __ldcs(reinterpret_cast<const float4*>(g) + v);
         const float4 w4 = reinterpret_cast<const float4*>(w)[v];
-        float4 s4[NS];
+        float4 s4[NA];
 #pragma unroll
         for (int k = 0; k < NS; ++k) s4[k] = reinterpret_cast<const float4*>(s[k])[v];
         const float gx[4] = {g4.x, g4.y, g4.z, g4.w}, wx[4] = {w4.x, w4.y, w4.z, w4.w};
-        float o[4], sx[NS][4];
+        float o[4], sx[NA][4];
 #pragma unroll
         for (int k = 0; k < NS; ++k) {
           sx[k][0] = s4[k].x; sx[k][1] = s4[k].y; sx[k][2] = s4[k].z; sx[k][3] = s4[k].w;
@@ -689,82 +643,13 @@ __global__ void bm_emit_pull_kernel(const uint32_t* bitmap, const uint32_t* pref
 }
 
 // ---------------------------------------------------------------------------------------------
-// standard (non-lazy) updates: EVERY weight row moves (weight decay / momentum / Adam moments),
-// rows absent from the gradient see grad = 0 (optimizer_op-inl.h:505-528, optimizer_op.cc:108-139,
-// 195-229). row_map[r] = position of row r in the gradient, or -1.
+// the row map of a row_sparse gradient for the updates that move EVERY table row
+// (update_rsp_grad_kernels.cu): row_map[r] = position of row r in the gradient, or -1
 
 __global__ void row_map_scatter_kernel(const int64_t* gidx, int64_t nnr, int32_t* row_map) {
   for (int64_t i = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x; i < nnr;
        i += static_cast<int64_t>(gridDim.x) * blockDim.x) {
     row_map[gidx[i]] = static_cast<int32_t>(i);
-  }
-}
-
-// AdamStdDnsRspDnsKernel<req,cpu> (optimizer_op.cc:195-229): absent rows use g' = w*wd, and the
-// variance squares first -- (1-beta2)*(g'*g') -- with or without clipping
-__device__ __forceinline__ float step_adam_std(float w, float g, bool present, float& s1, float& s2,
-                                               const Hyper& h) {
-  float gr = present ? __fadd_rn(__fmul_rn(g, h.rescale), __fmul_rn(w, h.wd)) : __fmul_rn(w, h.wd);
-  if (h.clip >= 0.f) gr = clipf(gr, h.clip);
-  s1 = __fadd_rn(__fmul_rn(h.beta1, s1), __fmul_rn(__fsub_rn(1.f, h.beta1), gr));
-  s2 = __fadd_rn(__fmul_rn(h.beta2, s2), __fmul_rn(__fsub_rn(1.f, h.beta2), __fmul_rn(gr, gr)));
-  return __fsub_rn(w, __fdiv_rn(__fmul_rn(h.lr, s1), __fadd_rn(__fsqrt_rn(s2), h.eps)));
-}
-
-template <int OPT>
-__global__ void __launch_bounds__(kWarpsPerBlock * 32) rsp_std_update_kernel(RspUpdateLaunch p,
-                                                                             const int32_t* row_map,
-                                                                             int64_t table_rows) {
-  const int64_t row = static_cast<int64_t>(blockIdx.x) * kWarpsPerBlock + (threadIdx.x >> 5);
-  if (row >= table_rows) return;
-  const int lane = threadIdx.x & 31;
-  Hyper h{p.lr, p.wd, p.momentum, p.rescale, p.clip, p.beta1, p.beta2, p.eps};
-  const int32_t gi = row_map[row];
-  const bool present = gi >= 0;
-  float* w = p.w + row * p.row_len;
-  float* s1 = p.s1 ? p.s1 + row * p.row_len : nullptr;
-  float* s2 = p.s2 ? p.s2 + row * p.row_len : nullptr;
-  const float* g = present ? p.gval + static_cast<int64_t>(gi) * p.row_len : nullptr;
-  auto one = [&](float wv, float gv, float& a, float& b) -> float {
-    if (OPT == kOptAdam) return step_adam_std(wv, gv, present, a, b, h);
-    if (OPT == kOptSGD) return step<kOptSGD>(wv, gv, a, b, true, h);  // grad = 0 when absent
-    // sgd_update: the whole weight is scaled by (1 - lr*wd); present rows then take the
-    // SGDDnsRspKernel step with wd = 0, i.e. (1.f - lr*0.f)*w' - ... = w' - ...
-    const float scaled = __fmul_rn(wv, __fsub_rn(1.f, __fmul_rn(h.lr, h.wd)));
-    if (!present) return scaled;
-    if (h.clip >= 0.f) return __fsub_rn(scaled, __fmul_rn(h.lr, clipf(__fmul_rn(h.rescale, gv), h.clip)));
-    return __fsub_rn(scaled, __fmul_rn(__fmul_rn(h.lr, h.rescale), gv));
-  };
-  const bool vec = (p.row_len % 4 == 0) && ((reinterpret_cast<uintptr_t>(p.w) & 15) == 0) &&
-                   ((reinterpret_cast<uintptr_t>(p.gval) & 15) == 0) &&
-                   (!p.s1 || (reinterpret_cast<uintptr_t>(p.s1) & 15) == 0) &&
-                   (!p.s2 || (reinterpret_cast<uintptr_t>(p.s2) & 15) == 0);
-  if (vec) {
-    const int64_t nv = p.row_len / 4;
-    for (int64_t v = lane; v < nv; v += 32) {
-      float4 wv = reinterpret_cast<float4*>(w)[v];
-      const float4 gv = present ? __ldcs(reinterpret_cast<const float4*>(g) + v)
-                                : make_float4(0.f, 0.f, 0.f, 0.f);
-      float4 a = make_float4(0, 0, 0, 0), b = make_float4(0, 0, 0, 0);
-      if (OPT == kOptSGD || OPT == kOptAdam) a = reinterpret_cast<float4*>(s1)[v];
-      if (OPT == kOptAdam) b = reinterpret_cast<float4*>(s2)[v];
-      wv.x = one(wv.x, gv.x, a.x, b.x);
-      wv.y = one(wv.y, gv.y, a.y, b.y);
-      wv.z = one(wv.z, gv.z, a.z, b.z);
-      wv.w = one(wv.w, gv.w, a.w, b.w);
-      reinterpret_cast<float4*>(w)[v] = wv;
-      if (OPT == kOptSGD || OPT == kOptAdam) reinterpret_cast<float4*>(s1)[v] = a;
-      if (OPT == kOptAdam) reinterpret_cast<float4*>(s2)[v] = b;
-    }
-  } else {
-    for (int64_t j = lane; j < p.row_len; j += 32) {
-      float a = 0.f, b = 0.f;
-      if (OPT == kOptSGD || OPT == kOptAdam) a = s1[j];
-      if (OPT == kOptAdam) b = s2[j];
-      w[j] = one(w[j], present ? g[j] : 0.f, a, b);
-      if (OPT == kOptSGD || OPT == kOptAdam) s1[j] = a;
-      if (OPT == kOptAdam) s2[j] = b;
-    }
   }
 }
 
@@ -1099,18 +984,6 @@ int GridFor(int64_t n, int threads) {
 
 }  // namespace
 
-void LaunchRspUpdate(const RspUpdateLaunch& p, cudaStream_t stream) {
-  if (p.nrows <= 0 || p.row_len <= 0) return;
-  const int blocks = static_cast<int>((p.nrows + kWarpsPerBlock - 1) / kWarpsPerBlock);
-  switch (p.opt) {
-    case kOptSGDSingle: rsp_update_kernel<kOptSGDSingle><<<blocks, kWarpsPerBlock * 32, 0, stream>>>(p); break;
-    case kOptSGD: rsp_update_kernel<kOptSGD><<<blocks, kWarpsPerBlock * 32, 0, stream>>>(p); break;
-    case kOptAdam: rsp_update_kernel<kOptAdam><<<blocks, kWarpsPerBlock * 32, 0, stream>>>(p); break;
-    default: KV_FATAL << "row_sparse update: unsupported optimizer kind " << p.opt;
-  }
-  KV_CUDA(cudaGetLastError());
-}
-
 void LaunchRspRowUpdateOp(const UpdateLaunch& L, cudaStream_t stream) {
   if (L.nnr <= 0 || L.row_len <= 0) return;
   KV_CHECK_EQ(L.dtype, kFloat32) << "row_sparse optimizer operators run on float32 arrays";
@@ -1132,9 +1005,15 @@ void LaunchRspRowUpdateOp(const UpdateLaunch& L, cudaStream_t stream) {
     return;
   }
   for (int k = 0; k < NumStates(L.op); ++k) vec = vec && aligned(L.s[k]);
+  // one warp per gradient row: CTAs that retire are replaced until the last row, where a capped
+  // grid of 40-56-register CTAs (6 or fewer resident per SM) leaves its last wave part empty
+  const int row_blocks = static_cast<int>((L.nnr + kWarpsPerBlock - 1) / kWarpsPerBlock);
   switch (L.op) {
-    case kUpdFtrl: rsp_row_update_kernel<kUpdFtrl><<<blocks, kWarpsPerBlock * 32, 0, stream>>>(L, vec); break;
-    case kUpdAdaGrad: rsp_row_update_kernel<kUpdAdaGrad><<<blocks, kWarpsPerBlock * 32, 0, stream>>>(L, vec); break;
+    case kUpdFtrl: rsp_row_update_kernel<kUpdFtrl><<<row_blocks, kWarpsPerBlock * 32, 0, stream>>>(L, vec); break;
+    case kUpdAdaGrad: rsp_row_update_kernel<kUpdAdaGrad><<<row_blocks, kWarpsPerBlock * 32, 0, stream>>>(L, vec); break;
+    case kUpdSGD: rsp_row_update_kernel<kUpdSGD><<<row_blocks, kWarpsPerBlock * 32, 0, stream>>>(L, vec); break;
+    case kUpdSGDMom: rsp_row_update_kernel<kUpdSGDMom><<<row_blocks, kWarpsPerBlock * 32, 0, stream>>>(L, vec); break;
+    case kUpdAdamLazy: rsp_row_update_kernel<kUpdAdamLazy><<<row_blocks, kWarpsPerBlock * 32, 0, stream>>>(L, vec); break;
     default: KV_FATAL << "row_sparse optimizer operator: unsupported operator " << L.op;
   }
   KV_CUDA(cudaGetLastError());
@@ -1303,20 +1182,6 @@ void LaunchRowMap(const int64_t* gidx, int64_t nnr, int64_t table_rows, int32_t*
     row_map_scatter_kernel<<<GridFor(nnr, 256), 256, 0, stream>>>(gidx, nnr, row_map);
     KV_CUDA(cudaGetLastError());
   }
-}
-
-void LaunchRspStdUpdate(const RspUpdateLaunch& p, int64_t table_rows, const int32_t* row_map,
-                        cudaStream_t stream) {
-  if (table_rows <= 0 || p.row_len <= 0) return;
-  const int blocks = static_cast<int>((table_rows + kWarpsPerBlock - 1) / kWarpsPerBlock);
-  const int threads = kWarpsPerBlock * 32;
-  switch (p.opt) {
-    case kOptSGDSingle: rsp_std_update_kernel<kOptSGDSingle><<<blocks, threads, 0, stream>>>(p, row_map, table_rows); break;
-    case kOptSGD: rsp_std_update_kernel<kOptSGD><<<blocks, threads, 0, stream>>>(p, row_map, table_rows); break;
-    case kOptAdam: rsp_std_update_kernel<kOptAdam><<<blocks, threads, 0, stream>>>(p, row_map, table_rows); break;
-    default: KV_FATAL << "standard row_sparse update: unsupported optimizer kind " << p.opt;
-  }
-  KV_CUDA(cudaGetLastError());
 }
 
 size_t NonzeroRowsWorkspaceBytes(int64_t rows) {

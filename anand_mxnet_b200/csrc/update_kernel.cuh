@@ -1,7 +1,8 @@
 // update_kernel.cuh -- the elementwise kernel of the single-tensor optimizer operators, shared by
 // update_kernels.cu (dense gradients: nag_mom_update / mp_nag_mom_update, signsgd_update /
 // signum_update, rmsprop_update / rmspropalex_update, ftml_update, ftrl_update) and
-// update_rsp_grad_kernels.cu (the same float32 operators with a row_sparse gradient).
+// update_rsp_grad_kernels.cu (the same float32 operators with a row_sparse gradient, and the
+// standard forms of sgd_update, sgd_mom_update and adam_update).
 //
 // One elementwise kernel update_kernel<OP, T, RSPG> over one flat tensor: a grid-stride loop whose
 // body moves 16 bytes per operand (float4, or 8 x 16 bit) when every operand is 16-byte aligned, and
@@ -70,12 +71,13 @@ __device__ __forceinline__ void StoreF(float* p, size_t v, const float (&x)[V]) 
   }
 }
 
-// the gradient of the V elements of 16-byte group v (RSPG: float32, row_len % V == 0, so one row)
+// the gradient of the V elements of 16-byte group v (RSPG: float32, row_len % V == 0, so one row);
+// returns whether that row is stored in the gradient (always, without RSPG)
 template <typename T, int V, bool RSPG>
-__device__ __forceinline__ void LoadGrad(const UpdateLaunch& a, size_t v, float (&g)[V]) {
+__device__ __forceinline__ bool LoadGrad(const UpdateLaunch& a, size_t v, float (&g)[V]) {
   if (!RSPG) {
     LoadT<T, V>(a.g, v, g);
-    return;
+    return true;
   }
   const size_t i = v * V;
   const size_t r = i / a.row_len;
@@ -83,15 +85,18 @@ __device__ __forceinline__ void LoadGrad(const UpdateLaunch& a, size_t v, float 
   if (gi < 0) {
 #pragma unroll
     for (int j = 0; j < V; ++j) g[j] = 0.f;
-    return;
+    return false;
   }
   LoadF<V>(static_cast<const float*>(a.g) + static_cast<size_t>(gi) * a.row_len + (i - r * a.row_len), 0, g);
+  return true;
 }
 template <typename T, bool RSPG>
-__device__ __forceinline__ float GradAt(const UpdateLaunch& a, size_t i) {
+__device__ __forceinline__ float GradAt(const UpdateLaunch& a, size_t i, bool& present) {
+  present = true;
   if (!RSPG) return ToF<T>(static_cast<const T*>(a.g)[i]);
   const size_t r = i / a.row_len;
   const int32_t gi = a.row_map[r];
+  present = gi >= 0;
   return gi < 0 ? 0.f : static_cast<const float*>(a.g)[static_cast<size_t>(gi) * a.row_len + (i - r * a.row_len)];
 }
 
@@ -105,7 +110,7 @@ __global__ void __launch_bounds__(kThreads) update_kernel(const UpdateLaunch a, 
   for (size_t v = tid; v < nv; v += stride) {
     float w[V], g[V], st[3][V], o[V];
     if (ReadsWeight(OP)) LoadT<T, V>(a.w, v, w);
-    LoadGrad<T, V, RSPG>(a, v, g);
+    const bool present = LoadGrad<T, V, RSPG>(a, v, g);
 #pragma unroll
     for (int k = 0; k < NS; ++k) LoadF<V>(a.s[k], v, st[k]);
 #pragma unroll
@@ -113,7 +118,7 @@ __global__ void __launch_bounds__(kThreads) update_kernel(const UpdateLaunch a, 
       float s[3] = {0.f, 0.f, 0.f};
 #pragma unroll
       for (int k = 0; k < NS; ++k) s[k] = st[k][j];
-      o[j] = Step<OP>(a, ReadsWeight(OP) ? w[j] : 0.f, g[j], s);
+      o[j] = Step<OP>(a, ReadsWeight(OP) ? w[j] : 0.f, g[j], s, present);
 #pragma unroll
       for (int k = 0; k < NS; ++k) st[k][j] = s[k];
     }
@@ -127,7 +132,9 @@ __global__ void __launch_bounds__(kThreads) update_kernel(const UpdateLaunch a, 
     float s[3] = {0.f, 0.f, 0.f};
 #pragma unroll
     for (int k = 0; k < NS; ++k) s[k] = a.s[k][i];
-    const float r = Step<OP>(a, ReadsWeight(OP) ? ToF<T>(w[i]) : 0.f, GradAt<T, RSPG>(a, i), s);
+    bool present;
+    const float g = GradAt<T, RSPG>(a, i, present);
+    const float r = Step<OP>(a, ReadsWeight(OP) ? ToF<T>(w[i]) : 0.f, g, s, present);
     out[i] = FromF<T>(r);
 #pragma unroll
     for (int k = 0; k < NS; ++k) a.s[k][i] = s[k];
@@ -144,7 +151,9 @@ void Launch(const UpdateLaunch& L, cudaStream_t stream) {
   if (RSPG) vec = vec && L.row_len % V == 0;  // a 16-byte group never straddles two rows
   const size_t items = vec ? (L.n / V + L.n % V) : L.n;
   const size_t want = (items + kThreads - 1) / kThreads;
-  const int grid = static_cast<int>(std::max<size_t>(1, std::min<size_t>(want, kNumSMs * 8)));
+  // RSPG: one thread per item, as the table-wide pass runs 30-56-register CTAs of which a capped
+  // grid would leave part of its last wave empty
+  const int grid = static_cast<int>(std::max<size_t>(1, RSPG ? want : std::min<size_t>(want, kNumSMs * 8)));
   update_kernel<OP, T, RSPG><<<grid, kThreads, 0, stream>>>(L, vec);
   KV_CUDA(cudaGetLastError());
 }

@@ -139,43 +139,16 @@ void RspUpdateOp(const Spec& spec, const std::vector<NDArray>& in, std::vector<N
       KV_CHECK(a.shape() == w.shape()) << n << ": weight / grad / state shape mismatch";
     }
   }
-  // CheckAllRowsPresent (operator_common.h:500-511)
-  const char* func = op == kUpdFtrl ? "FtrlUpdate" : op == kUpdAdaGrad ? "AdagradUpdate" : "GroupAdagradUpdate";
-  KV_CHECK(wst != kRowSparseStorage || w.nnr() == rows)
-      << func << " for RowSparse weights is only implemented for RowSparse weights with all rows "
-      << "containing non-zeros. Expects weights.data.shape[0] (" << w.nnr() << ") == weights.shape[0] ("
-      << rows << ").";
   // the states' rows are addressed by the table row id, like the weight's: a row_sparse state holds
-  // every row, or none yet (then it is zero-filled first, FillDnsZerosRspImpl)
-  for (size_t i = 2; i < in.size(); ++i) {
-    KV_CHECK(in[i].stype() != kRowSparseStorage || in[i].nnr() == 0 || in[i].nnr() == rows)
-        << n << ": a row_sparse optimizer state must hold every row or none (it holds "
-        << in[i].nnr() << " of " << rows << ")";
-  }
-  // kWriteInplace is expected (optimizer_op-inl.h:2235, 2572)
-  KV_CHECK(outputs->size() == 1 && (*outputs)[0].SameStorage(w) && (*outputs)[0].stype() == wst &&
-           (*outputs)[0].data() == w.data())
-      << n << ": out must be the weight itself (kWriteInplace is expected for sparse " << n << ")";
+  // every row, or none yet (then it is zero-filled first, FillDnsZerosRspImpl); kWriteInplace is
+  // expected (optimizer_op-inl.h:2235, 2572)
+  const char* func = op == kUpdFtrl ? "FtrlUpdate" : op == kUpdAdaGrad ? "AdagradUpdate" : "GroupAdagradUpdate";
+  CheckRspTable(n, func, in, *outputs);
 
   // a state with no rows is zero-filled even when the gradient is empty
-  ZeroFillEmptyRspStates(std::vector<NDArray>(in.begin() + 2, in.end()), rows, spec.launch_name);
-  if (!g.storage_initialized()) return;  // an all-zero gradient changes nothing
-  LaneOp lop(w.dev());
-  lop.Read(g).Write(w);
-  for (size_t i = 2; i < in.size(); ++i) lop.Write(in[i]);
-  L.w = w.data();
-  L.out = w.data();
-  L.g = g.data();
-  L.gidx = g.row_ids();
-  L.nnr = g.nnr();
-  L.row_len = static_cast<int64_t>(w.RowLength());
-  for (size_t i = 2; i < in.size(); ++i) L.s[i - 2] = static_cast<float*>(in[i].data());
-  LaunchRspRowUpdateOp(L, lop.stream());
-  // + 8 B of id per row, and GroupAdaGrad's history value read and written
-  const int64_t per_row = op == kUpdGroupAdaGrad ? 16 : 8;
-  Engine::Get()->CountLaunch(spec.launch_name,
-                             static_cast<uint64_t>(L.nnr) * (spec.bytes_per_elem * L.row_len + per_row));
-  lop.Issue();
+  const std::vector<NDArray> states(in.begin() + 2, in.end());
+  ZeroFillEmptyRspStates(states, rows, spec.launch_name);
+  RunRspRowUpdate(L, w, g, states, spec.launch_name, spec.bytes_per_elem);
 }
 
 std::string Stypes(const std::vector<NDArray>& in) {
@@ -292,6 +265,11 @@ void UpdateOp(const OpInfo& info, const std::vector<NDArray>& in, std::vector<ND
       L.beta = GetF(p, "beta", 1.0f);
       break;
   }
+  if (rsp_grad) {
+    RunRspGradUpdate(L, w, g, std::vector<NDArray>(in.begin() + 2, in.end()), out, spec.rsp_grad_launch_name,
+                     spec.bytes_per_elem);
+    return;
+  }
   L.w = w.data();
   L.g = g.data();
   L.out = out.data();
@@ -304,28 +282,8 @@ void UpdateOp(const OpInfo& info, const std::vector<NDArray>& in, std::vector<ND
   if (!out_is_w) lop.Read(w);
   lop.Write(out);
   for (int i = 2; i < spec.nin; ++i) lop.Write(in[i]);
-  if (!rsp_grad) {
-    LaunchUpdateOp(L, lop.stream());
-    Engine::Get()->CountLaunch(spec.launch_name, static_cast<uint64_t>(spec.bytes_per_elem) * L.n);
-    lop.Issue();
-    return;
-  }
-  // the stored rows through a row map, every element of the table updated; an empty gradient is
-  // a full update with g = +0.0f
-  const int64_t rows = w.shape()[0];
-  const NDArray row_map = BuildRowMap(lop, g, rows);
-  L.g = g.storage_initialized() ? g.data() : nullptr;
-  L.nnr = g.nnr();
-  L.row_len = static_cast<int64_t>(w.RowLength());
-  L.row_map = static_cast<const int32_t*>(row_map.data());
-  LaunchRspGradUpdateOp(L, lop.stream());
-  // bytes: the scatter reads an 8 B id and writes 4 B per stored row; the update moves the dense
-  // pass's bytes less the gradient's 4 B per element, reads the stored rows once, and counts the
-  // row map's memset and read (4 B each per table row)
-  if (L.nnr > 0) Engine::Get()->CountLaunch("update_op(row_map_scatter)", static_cast<uint64_t>(L.nnr) * 12);
-  Engine::Get()->CountLaunch(spec.rsp_grad_launch_name,
-                             static_cast<uint64_t>(spec.bytes_per_elem - 4) * L.n +
-                                 static_cast<uint64_t>(L.nnr) * L.row_len * 4 + static_cast<uint64_t>(rows) * 8);
+  LaunchUpdateOp(L, lop.stream());
+  Engine::Get()->CountLaunch(spec.launch_name, static_cast<uint64_t>(spec.bytes_per_elem) * L.n);
   lop.Issue();
 }
 

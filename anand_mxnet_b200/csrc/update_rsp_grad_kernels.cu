@@ -1,7 +1,8 @@
 // update_rsp_grad_kernels.cu -- nag_mom_update, signsgd_update, signum_update, rmsprop_update,
 // rmspropalex_update, ftml_update and ftrl_update with a dense float32 weight and states and a
-// row_sparse gradient: update_kernel<OP, float, true> (update_kernel.cuh) over the whole table,
-// reading the gradient's stored rows through the row map of LaunchRowMap.
+// row_sparse gradient, and the standard (lazy_update=False) forms of sgd_update, sgd_mom_update and
+// adam_update: update_kernel<OP, float, true> (update_kernel.cuh) over the whole table, reading the
+// gradient's stored rows through the row map of LaunchRowMap.
 #include "update_kernel.cuh"
 
 namespace b200kv {
@@ -18,6 +19,9 @@ void LaunchRspGradUpdateOp(const UpdateLaunch& L, cudaStream_t stream) {
     case kUpdRMSPropAlex: Launch<kUpdRMSPropAlex, float, true>(L, stream); break;
     case kUpdFTML: Launch<kUpdFTML, float, true>(L, stream); break;
     case kUpdFtrl: Launch<kUpdFtrl, float, true>(L, stream); break;
+    case kUpdSGDStd: Launch<kUpdSGDStd, float, true>(L, stream); break;
+    case kUpdSGDMom: Launch<kUpdSGDMom, float, true>(L, stream); break;
+    case kUpdAdamStd: Launch<kUpdAdamStd, float, true>(L, stream); break;
     default: KV_FATAL << "operator " << L.op << " has no row_sparse-gradient form";
   }
 }

@@ -1,26 +1,33 @@
 #!/usr/bin/env python
-"""bench_sparse_sgd_adam.py -- lazy sgd_mom_update and adam_update on a row_sparse weight that holds
-every row (rowsparse_kernels.cu: rsp_update_kernel), on one GPU, on an embedding table of
+"""bench_sparse_sgd_adam.py -- sgd_mom_update and adam_update with a row_sparse gradient: the lazy
+form on a row_sparse weight that holds every row and on a dense weight (rowsparse_kernels.cu:
+rsp_row_update_kernel), and the standard form on a dense weight (update_rsp_grad_kernels.cu:
+update_kernel<OP, float, true> after the row map), on one GPU, on an embedding table of
 --rows x --row-len float32 (default 1 M x 512) with --nnr (default 1 % of the rows) seeded unique
 gradient rows.
 
 Workloads, each timed with CUDA events over --iters calls after --warmup:
   sgd_mom_rsp   sgd_mom_update, weight / grad / mom all row_sparse, lazy_update=True
   sgd_mom_dns   the same call on a dense weight and momentum: the same kernel, the same work
+  sgd_mom_std   the dense-weight call with lazy_update=False: every row of the table moves, rows
+                absent from the gradient with g = 0
   adam_rsp      adam_update, weight / grad / mean / var all row_sparse, lazy_update=True
   adam_dns      the same call on a dense weight, mean and var
+  adam_std      the dense-weight call with lazy_update=False
   state_fill    the first-use fill of one row_sparse state that holds no rows: all rows allocated,
                 zeroed and given ids 0..rows-1 (a sgd_mom_update with an empty gradient, which
                 changes nothing else); timed per call including a fresh empty state each time
 
 Before timing, the first call of every update workload is checked bit for bit against the C
 restatement of the reference's kernels (oracle/kvoracle.c, which the tests hold to the reference's
-own code) on the touched rows, and a sample of untouched rows is checked unchanged; the fill is
-checked to leave every row zero. The run fails if any differs. One JSON line per workload: time,
-algorithmic GB/s (bytes per touched element: SGD-momentum 20 = g 4 + w 8 + mom 8; Adam 28 = g 4 +
-w 8 + mean 8 + var 8; plus 8 bytes of id per row; the fill writes rows x (row_len x 4 + 8)) and its
-fraction of the 3.35 TB/s H100 SXM data-sheet bandwidth (a bound that was not measured), with the
-card's name and power limit.
+own code) on the touched rows and on a sample of untouched rows (unchanged by the lazy form); the
+fill is checked to leave every row zero. The run fails if any differs. One JSON line per workload:
+time, algorithmic GB/s (bytes per touched element: SGD-momentum 20 = g 4 + w 8 + mom 8; Adam 28 =
+g 4 + w 8 + mean 8 + var 8; plus 8 bytes of id per row. The standard form touches every table
+element without reading a gradient there, 4 bytes fewer, and reads the gradient's rows once and
+the row map, 8 bytes per table row and 4 per gradient row; the fill writes rows x (row_len x 4 +
+8)) and its fraction of the 3.35 TB/s H100 SXM data-sheet bandwidth (a bound that was not
+measured), with the card's name and power limit.
 """
 import argparse
 import ctypes
@@ -115,32 +122,43 @@ def main():
     gvals = uniform(-1, 1, N, L)
     g = rsp(gvals, ids)
     g_np = gvals.cpu().numpy()
-    for kind, params, nst in (('sgd_mom', SGD_MOM, 1), ('adam', ADAM, 2)):
+    for kind, lazy_params, nst in (('sgd_mom', SGD_MOM, 1), ('adam', ADAM, 2)):
         op = getattr(mx.nd.sparse, kind + '_update')
-        for stype in ('row_sparse', 'default'):
+        for stype, lazy in (('row_sparse', True), ('default', True), ('default', False)):
+            params = dict(lazy_params, lazy_update=lazy)
             w0 = uniform(-1, 1, R, L)
             s0 = [uniform(-0.1, 0.1, R, L), uniform(0, 0.01, R, L)][:nst]
             w = table(w0, stype)
             sts = [table(s, stype) for s in s0]
-            before = [t.index_select(0, ids).cpu().numpy() for t in [w0] + s0]
+            # the standard form moves every row: the touched rows (first) and the untouched sample
+            # form one sub-table for the oracle
+            checked = ids if lazy else torch.cat([ids, cold])
+            before = [t.index_select(0, checked).cpu().numpy() for t in [w0] + s0]
             op(w, g, *sts, out=w, **params)
             mx.nd.waitall()
             after = [tensor(a) for a in [w] + sts]
             kw = dict(lr=params['lr'], wd=params['wd'])
             if kind == 'sgd_mom':
-                oracle.sgd_mom_rsp_update(before[0], before[1], np.arange(N), g_np, momentum=0.9, **kw)
+                (oracle.sgd_mom_rsp_update if lazy else oracle.sgd_mom_std_rsp_update)(
+                    before[0], before[1], np.arange(N), g_np, momentum=0.9, **kw)
             else:
-                oracle.adam_rsp_update(*before, np.arange(N), g_np, **kw)
-            ok = all(np.array_equal(a.index_select(0, ids).cpu().numpy().view(np.uint32), b.view(np.uint32))
+                (oracle.adam_rsp_update if lazy else oracle.adam_std_rsp_update)(*before, np.arange(N), g_np, **kw)
+            ok = all(np.array_equal(a.index_select(0, checked).cpu().numpy().view(np.uint32), b.view(np.uint32))
                      for a, b in zip(after, before))
-            ok = ok and all(torch.equal(a.index_select(0, cold).view(torch.int32), b.index_select(0, cold).view(torch.int32))
-                            for a, b in zip(after, [w0] + s0))
-            workload = "%s_%s" % (kind, 'rsp' if stype == 'row_sparse' else 'dns')
+            if lazy:
+                ok = ok and all(torch.equal(a.index_select(0, cold).view(torch.int32),
+                                            b.index_select(0, cold).view(torch.int32))
+                                for a, b in zip(after, [w0] + s0))
+            workload = "%s_%s" % (kind, 'std' if not lazy else 'rsp' if stype == 'row_sparse' else 'dns')
             print(json.dumps({"parity": workload, "bit_exact": bool(ok)}), flush=True)
             if not ok:
                 failed.append(workload)
             ms = timed(lambda: op(w, g, *sts, out=w, **params))
-            emit(workload, N * (BYTES[kind] * L + 8), ms, {"weight_stype": stype})
+            if lazy:
+                nbytes = N * (BYTES[kind] * L + 8)
+            else:
+                nbytes = R * L * (BYTES[kind] - 4) + N * (L * 4 + 8 + 4) + R * 8
+            emit(workload, nbytes, ms, {"weight_stype": stype, "lazy_update": lazy})
             del w, sts, after, w0, s0
             torch.cuda.empty_cache()
     # first-use fill of one row_sparse momentum that holds no rows

@@ -79,13 +79,14 @@ def test_trajectories_vs_reference_live(golden):
             assert RRG.OPLOG == gold['%s|log' % name].tolist()
 
 
-def test_ptxas_no_spills_rsp_grad(tmp_path):
-    """the seven row_sparse-gradient kernels compile for sm_90a with no spills and no stack frame"""
+def test_ptxas_no_spills_rsp_grad_and_std_sgd_adam(tmp_path):
+    """the ten row_sparse-gradient kernels (seven operators and the standard sgd_update, sgd_mom_update
+    and adam_update forms) compile for sm_90a with no spills and no stack frame"""
     from anand_mxnet_b200 import build as B
     src = os.path.join(B.CSRC, "update_rsp_grad_kernels.cu")
     r = subprocess.run([B._nvcc()] + B.NVCC_FLAGS + ["-Xptxas", "-v", "-c", src, "-o", str(tmp_path / "u.o")],
                        capture_output=True, text=True, env=B._env())
     assert r.returncode == 0, r.stderr[-4000:]
     frames = re.findall(r"(\d+) bytes stack frame, (\d+) bytes spill stores, (\d+) bytes spill loads", r.stderr)
-    assert len(frames) == 7, r.stderr[-4000:]
+    assert len(frames) == 10, r.stderr[-4000:]
     assert all(f == ('0', '0', '0') for f in frames), frames

@@ -105,6 +105,31 @@ def test_rsp_weight_equals_dense_weight(mx):
         assert eq(a.asnumpy(), b.asnumpy()) and eq(ma.asnumpy(), mb.asnumpy()) and eq(va.asnumpy(), vb.asnumpy())
 
 
+@pytest.mark.parametrize("wst", ['default', 'row_sparse'])
+def test_adam_std_absent_row_is_not_a_zero_row(mx, oracle, wst):
+    """the standard Adam form tells a row absent from the gradient from a stored row of zeros
+    (AdamStdDnsRspDnsKernel, optimizer_op.cc:195-229): with negative weights and wd = 0 an absent
+    row's g' = w*wd is -0.0 and keeps a mean of -0.0, where g*rescale + w*wd with g = +0.0f would
+    make it +0.0. Bit for bit against the C restatement of the reference's kernel."""
+    import kvoracle as K
+    rng = np.random.default_rng(5)
+    shape = (23, 5)
+    w0 = -rng.uniform(0.1, 1, shape).astype(np.float32)
+    m0 = np.full(shape, -0.0, np.float32)
+    v0 = rng.uniform(0, 0.01, shape).astype(np.float32)
+    ids = np.array([2, 7, 11, 20], np.int64)
+    g = rng.uniform(-1, 1, (len(ids), 5)).astype(np.float32)
+    w = mx.nd.array(w0, mx.gpu(0)) if wst == 'default' else rsp(mx, w0, np.arange(23), shape)
+    m, v = mx.nd.array(m0, mx.gpu(0)), mx.nd.array(v0, mx.gpu(0))
+    mx.nd.sparse.adam_update(w, rsp(mx, g, ids, shape), m, v, out=w, lr=0.01, wd=0.0, lazy_update=False)
+    want = [w0.copy(), m0.copy(), v0.copy()]
+    oracle.adam_std_rsp_update(*want, ids, g, K.scalar_param(0.01), wd=0.0)
+    absent = np.setdiff1d(np.arange(23), ids)
+    assert np.all(np.signbit(want[1][absent])) and np.all(want[1][absent] == 0)
+    for got, ref in zip((w, m, v), want):
+        assert eq(got.asnumpy(), ref)
+
+
 # ------------------------------------------------------------------------------------ refusals
 def _untouched(mx, call_, arrays):
     before = [(a.asnumpy().copy(), nnr(a)) for a in arrays]

@@ -164,8 +164,9 @@ def test_compat_adagrad_dense_gradient_is_refused():
         opt.update(0, Dense(), Dense(), None)
 
 
-def test_ptxas_no_spills(tmp_path):
-    """the two row-gather instantiations (and the id fill) of rowsparse_kernels.cu"""
+def test_ptxas_no_spills_row_updates(tmp_path):
+    """the five row-gather instantiations (Ftrl, AdaGrad, lazy SGD, SGD-momentum and Adam) and the id
+    fill of rowsparse_kernels.cu: no spills, no stack frame"""
     from anand_mxnet_b200 import build as B
     src = os.path.join(B.CSRC, "rowsparse_kernels.cu")
     r = subprocess.run([B._nvcc()] + B.NVCC_FLAGS + ["-Xptxas", "-v", "-c", src, "-o",
@@ -173,7 +174,8 @@ def test_ptxas_no_spills(tmp_path):
                        capture_output=True, text=True, env=B._env())
     assert r.returncode == 0, r.stderr[-4000:]
     blocks = re.split(r"Compiling entry function ", r.stderr)[1:]   # one per kernel
-    found = [(b.split("'")[1],) + re.search(r"(\d+) bytes spill stores, (\d+) bytes spill loads", b).groups()
+    found = [(b.split("'")[1],) + re.search(r"(\d+) bytes stack frame, (\d+) bytes spill stores, "
+                                            r"(\d+) bytes spill loads", b).groups()
              for b in blocks if re.match(r"'\w*(rsp_row_update_kernel|fill_row_ids_kernel)", b)]
-    assert len(found) == 3, r.stderr[-4000:]
-    assert all(s == '0' and l == '0' for _, s, l in found), found
+    assert len(found) == 6, r.stderr[-4000:]
+    assert all(f == '0' and s == '0' and l == '0' for _, f, s, l in found), found
