@@ -288,6 +288,18 @@ static_assert(sizeof(ResetArraysList) <= 32764, "kernel parameters are limited t
 // reset_arrays_kernel: one launch, none when every array is empty. Returns the number of launches.
 int LaunchResetArrays(ResetArraysList& arrays, cudaStream_t stream);
 
+// add_n / ElementWiseSum on dense arrays (tensor/elemwise_sum.h:48-98, ElementWiseSumCompute_):
+// out = in[0] + (in[1] + (in[2] + in[3])) for 2-4 inputs, else the left chain out = in[0], then
+// out = out + in[i]. Every + is in the dtype: the 16-bit types add in float and round once, integers
+// wrap. zero_first starts the chain at +0 (out = 0 + in[0] + ...: ElementwiseSumContainsDnsImpl
+// with a row_sparse in[0]). The input list travels by value, up to kAddNMaxArrays per launch; past
+// that the chain continues in the next launch from out. Any alignment; out may be in[0] itself.
+// float16, bfloat16, float32, float64, uint8, int8, int32 and int64 (sum_kernels.cu). Returns the
+// number of launches: none for an empty out, else ceil((n_in - 1) / (kAddNMaxArrays - 1)), at least 1.
+constexpr int kAddNMaxArrays = 200;
+int LaunchAddN(int dtype, const void* const* in, int n_in, bool zero_first, void* out, uint64_t n,
+               cudaStream_t stream);
+
 // ---- single-tensor optimizer operators of the callback route (update_kernels.cu) ----
 // nag_mom_update, mp_nag_mom_update, signsgd_update, signum_update, rmsprop_update,
 // rmspropalex_update, ftml_update, ftrl_update (optimizer_op-inl.h:1061-1222, 1953-2158, 2344-2431).

@@ -539,6 +539,52 @@ void SgdAdamRspUpdate(int kind, bool lazy, UpdateLaunch L, const NDArray& w, con
   }
 }
 
+void SumRowSparse(const std::vector<NDArray>& in, const NDArray& out) {
+  const int dev = out.dev();
+  Engine* eng = Engine::Get();
+  std::vector<NDArray> srcs;
+  bool out_is_input = false;
+  for (const NDArray& a : in) {
+    out_is_input = out_is_input || a.SameStorage(out);
+    if (a.storage_initialized()) srcs.push_back(a);
+  }
+  if (srcs.empty()) {  // every input is all zeros: out stores no rows, nothing is launched
+    LaneOp op(dev);
+    op.Write(out);
+    op.Issue();
+    out.SetNnr(0);
+    return;
+  }
+  const int bits = BitsFor(out.shape()[0]);
+  const int64_t row_len = static_cast<int64_t>(out.RowLength());
+  NDArray acc;  // the sum so far
+  for (size_t next = 0; next < srcs.size();) {
+    std::vector<NDArray> group;
+    if (!acc.is_none()) group.push_back(acc);
+    while (group.size() < static_cast<size_t>(kMaxSrc) && next < srcs.size()) group.push_back(srcs[next++]);
+    const bool last = next == srcs.size();
+    const NDArray target = last && !out_is_input ? out : NDArray::RowSparse(out.shape(), Context::GPU(dev), kFloat32);
+    const RspSources S = LocalSources(group);
+    const int64_t total = S.start[S.nsrc];
+    target.CheckAndAllocRows(total);  // upper bound; nnr is set once the count is known
+    NDArray d_nnr({1}, Context::GPU(dev), kInt64);
+    NDArray ws({static_cast<int64_t>(RspMergeWorkspaceBytes(total, bits, S.nsrc))}, Context::GPU(dev), kUint8);
+    LaneOp op(dev);
+    for (const NDArray& g : group) op.Read(g);
+    op.Write(target).Write(d_nnr).Write(ws);
+    LaunchRspMerge(S, bits, row_len, target.row_ids(), static_cast<float*>(target.data()),
+                   static_cast<int64_t*>(d_nnr.data()), ws.data(), ws.ByteSize(), op.stream());
+    eng->CountLaunch("rsp_merge(tag, sort, heads)", total * 24);
+    eng->CountLaunch("rsp_sum", static_cast<uint64_t>(total) * row_len * 4 * 2);
+    op.Issue();
+    CountFence f(dev, 1);
+    f.Post(static_cast<const int64_t*>(d_nnr.data()), op.stream());
+    target.SetNnr(f.Wait()[0]);
+    acc = target;
+  }
+  if (!acc.SameStorage(out)) CopyFromTo(acc, out);
+}
+
 void CastStorageCopy(const NDArray& from_in, const NDArray& to) {
   KV_CHECK(from_in.stype() == kDefaultStorage || to.stype() == kDefaultStorage)
       << "Copying ndarray of stype = " << from_in.stype() << " to stype = " << to.stype()

@@ -34,6 +34,14 @@ void SgdAdamRspUpdate(int kind, bool lazy, UpdateLaunch L, const NDArray& w, con
 // its stream, so it is called after every other operand of `op` is declared.
 NDArray BuildRowMap(LaneOp& op, const NDArray& g, int64_t rows);
 
+// add_n of row_sparse float32 arrays on out's GPU (ElementwiseSumRsp, ndarray_function.cc:60-176):
+// out holds the sorted union of the inputs' row ids, each row +0.0f plus the inputs that hold it in
+// input order. The store's merge (LaunchRspMerge without an update) over up to kMaxSrc inputs at a
+// time; past that the partial sum is the first source of the next merge, which is bit-identical
+// (+0.0f + a partial row is that row: a partial sum is never -0.0f). out may be one of the inputs.
+// The caller has checked shapes, dtypes and devices. Waits on the host for the row count.
+void SumRowSparse(const std::vector<NDArray>& in, const NDArray& out);
+
 // CopyFromTo across storage types (src/ndarray/ndarray.cc:1147-1196 + cast_storage-inl.h:74-140):
 // dense -> row_sparse keeps the rows with a non-zero element, row_sparse -> dense scatters the
 // rows over zeros. float32 only; the cast runs on a GPU (the source's, else the target's).

@@ -582,6 +582,24 @@ multi_all_finite = _op('multi_all_finite')
 reset_arrays = _op('reset_arrays')
 # zeros of data's shape and dtype; a row_sparse data or out gives a row_sparse array with no rows
 zeros_like = _op('zeros_like')
+
+
+def _sum_op(name):
+    """add_n(*arrays, out=None): the element-wise sum of arrays of one shape and dtype on one GPU.
+    num_args is len(arrays) unless given, as the reference's generated function fills it in. Dense
+    inputs give a dense sum in the reference's association; row_sparse (float32) inputs a row_sparse
+    sum; a mix a dense one. out may be the first input itself."""
+    def f(*arrays, **kwargs):
+        out = kwargs.pop('out', None)
+        kwargs.setdefault('num_args', len(arrays))
+        return _invoke(name, list(arrays), out=out, **kwargs)
+    f.__name__ = name
+    return f
+
+
+add_n = _sum_op('add_n')
+ElementWiseSum = _sum_op('ElementWiseSum')
+_Sparse.add_n = staticmethod(_sum_op('_sparse_add_n'))
 preloaded_multi_sgd_update = _op('preloaded_multi_sgd_update')
 preloaded_multi_sgd_mom_update = _op('preloaded_multi_sgd_mom_update')
 preloaded_multi_mp_sgd_update = _op('preloaded_multi_mp_sgd_update')
