@@ -15,6 +15,7 @@ from .base import MXNetError
 from .context import Context, cpu, gpu, cpu_pinned
 from . import ndarray
 from . import ndarray as nd
+from . import random
 from . import optimizer
 from . import gluon
 from . import kvstore

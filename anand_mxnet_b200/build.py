@@ -40,13 +40,22 @@ def sources():
 
 def _newest_header():
     hs = [os.path.join(CSRC, f) for f in os.listdir(CSRC) if f.endswith(".h")]
-    hs.append(os.path.join(ROOT, "include", "b200kv_c_api.h"))
+    hs += [os.path.join(ROOT, "include", h) for h in ("b200kv_c_api.h", "b200kv_random_api.h")]
     return max(os.path.getmtime(h) for h in hs)
+
+
+def flags_for(src):
+    """The reference's GPU sampler is built with nvcc's default contraction, and curand's Box-Muller
+    arithmetic in its headers contracts with it: random_kernels.cu keeps -fmad=true to draw the same
+    numbers. Every other file keeps the CPU reference's -fmad=false."""
+    if src == "random_kernels.cu":
+        return ["-fmad=true" if f == "-fmad=false" else f for f in NVCC_FLAGS]
+    return NVCC_FLAGS
 
 
 def _compile(nvcc, src, verbose):
     obj = os.path.join(OBJ, src + ".o")
-    cmd = [nvcc] + NVCC_FLAGS + (["-Xptxas", "-v"] if verbose else []) + \
+    cmd = [nvcc] + flags_for(src) + (["-Xptxas", "-v"] if verbose else []) + \
         ["-c", os.path.join(CSRC, src), "-o", obj]
     r = subprocess.run(cmd, capture_output=True, text=True, env=_env())
     if r.returncode != 0:

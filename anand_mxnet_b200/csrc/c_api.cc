@@ -25,6 +25,7 @@
 #include "nccl_dyn.h"
 #include "ndarray.h"
 #include "ops.h"
+#include "random_ops.h"
 #include "scalar_parse.h"
 
 using namespace b200kv;  // NOLINT
@@ -108,6 +109,18 @@ int MXGetGPUCount(int* out) {
 int MXNotifyShutdown(void) {
   API_BEGIN();
   Engine::Get()->Shutdown();
+  API_END();
+}
+
+int MXRandomSeed(int seed) {
+  API_BEGIN();
+  RandomSeed(static_cast<uint32_t>(seed));
+  API_END();
+}
+
+int MXRandomSeedContext(int seed, int dev_type, int dev_id) {
+  API_BEGIN();
+  RandomSeedContext(static_cast<uint32_t>(seed), MakeCtx(dev_type, dev_id));
   API_END();
 }
 
@@ -1022,6 +1035,19 @@ B200KV_DLL int B200KVTestNcclAvailable(int* available, char* version, size_t ver
     return HandleException(e);
   }
   return 0;
+}
+
+int B200KVRandomStates(int dev_id, int copy, void* out, size_t bytes) {
+  API_BEGIN();
+  RandomStates(dev_id, copy, out, bytes);
+  API_END();
+}
+
+int B200KVRandomNormalInto(NDArrayHandle out, float loc, float scale, int staged) {
+  API_BEGIN();
+  KVStore::FlushAll();
+  RandNormalInto(ND(out), loc, scale, staged != 0);
+  API_END();
 }
 
 int B200KVGetKernelLaunchCount(uint64_t* out) {

@@ -300,6 +300,21 @@ constexpr int kAddNMaxArrays = 200;
 int LaunchAddN(int dtype, const void* const* in, int n_in, bool zero_first, void* out, uint64_t n,
                cudaStream_t stream);
 
+// ---- the reference's GPU parallel sampler (random_kernels.cu; common/random_generator.cu,
+// random/sampler.h) ----
+// One generator copy is kRandStates curandStatePhilox4_32_10_t states of kRandStateBytes each.
+constexpr int kRandStates = 32768;
+constexpr int kRandMinPerThread = 64;
+constexpr int kRandStateBytes = 64;
+// state id = curand_init(seed, id, 0) for every id of the copy (one launch)
+void LaunchRandSeed(void* states, uint32_t seed, cudaStream_t stream);
+// out[i] = dtype(normal() * scale + loc) over n elements in LaunchRNG's state-to-element mapping,
+// advancing the copy's states (float16, bfloat16, float32, float64; any alignment). staged = false
+// stores as each thread draws, the reference's store order (for measurement only). No launch when
+// n == 0.
+void LaunchRandNormal(int dtype, void* states, void* out, uint64_t n, float loc, float scale, bool staged,
+                      cudaStream_t stream);
+
 // ---- single-tensor optimizer operators of the callback route (update_kernels.cu) ----
 // nag_mom_update, mp_nag_mom_update, signsgd_update, signum_update, rmsprop_update,
 // rmspropalex_update, ftml_update, ftrl_update (optimizer_op-inl.h:1061-1222, 1953-2158, 2344-2431).

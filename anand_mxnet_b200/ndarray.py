@@ -730,3 +730,15 @@ class _Contrib(object):
 
 
 contrib = _Contrib()
+
+
+class _Random(object):
+    """mx.nd.random: the samplers of mx.random (random.py)"""
+
+    @property
+    def normal(self):
+        from .random import normal as _normal
+        return _normal
+
+
+random = _Random()

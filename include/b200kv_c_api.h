@@ -297,4 +297,8 @@ B200KV_DLL const char* B200KVBuildInfo(void);
 #ifdef __cplusplus
 }
 #endif
+
+/* the random number generators (seeding, and the sampler's introspection) */
+#include "b200kv_random_api.h"
+
 #endif /* B200KV_C_API_H_ */
