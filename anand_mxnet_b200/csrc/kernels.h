@@ -314,6 +314,19 @@ void LaunchRandSeed(void* states, uint32_t seed, cudaStream_t stream);
 // n == 0.
 void LaunchRandNormal(int dtype, void* states, void* out, uint64_t n, float loc, float scale, bool staged,
                       cudaStream_t stream);
+// The scalar-parameter samplers of random/sampler.h, in the same mapping and staged store:
+//   kRandUniform      a + (b - a) * uniform()                  (low a, high b)
+//   kRandExponential  -log(1 - uniform()) / a                   (lam a)
+//   kRandGamma        Marsaglia-Tsang, shape a, scale b
+//   kRandInt          lo + rand_int64() % (hi - lo), hi > lo    (int32, int64)
+// The first three write float16, bfloat16, float32 or float64. No launch when n == 0.
+enum RandDist { kRandUniform, kRandExponential, kRandGamma, kRandInt };
+struct RandParams {
+  float a = 0.0f, b = 0.0f;
+  int64_t lo = 0, hi = 0;
+};
+void LaunchRandSample(int dist, int dtype, void* states, void* out, uint64_t n, const RandParams& p,
+                      cudaStream_t stream);
 
 // ---- single-tensor optimizer operators of the callback route (update_kernels.cu) ----
 // nag_mom_update, mp_nag_mom_update, signsgd_update, signum_update, rmsprop_update,

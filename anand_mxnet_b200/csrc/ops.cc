@@ -90,7 +90,8 @@ const OpInfo* FindOp(const std::string& name) {
   static const auto* table = [] {
     auto* m = new std::unordered_map<std::string, const OpInfo*>();
     for (const std::vector<OpInfo>* family :
-         {&kCoreOps, &kMultiTensorOps, &kUpdateOps, &kArithOps, &kReduceOps, &kSumOps, &kRandomOps}) {
+         {&kCoreOps, &kMultiTensorOps, &kUpdateOps, &kArithOps, &kReduceOps, &kSumOps, &kRandomOps,
+          &kSampleOps}) {
       for (const OpInfo& op : *family) {
         KV_CHECK(m->emplace(op.name, &op).second) << "operator " << op.name << " is declared twice";
       }

@@ -1,6 +1,7 @@
 // random_ops.cc -- the GPU parallel random generators (ResourceParallelRandom<gpu>, resource.cc:
-// 205-360), their seeding (MXRandomSeed / MXRandomSeedContext) and the sampling operator
-// _random_normal (random/sample_op.cc, SampleNormalParam and normal_op in sample_op.h).
+// 205-360), their seeding (MXRandomSeed / MXRandomSeedContext), the draw path every sampler takes
+// (SampleInto), and the sampling operator _random_normal (random/sample_op.cc, SampleNormalParam and
+// normal_op in sample_op.h). The other samplers' operators are in sample_ops.cc.
 //
 // Each GPU holds kRandCopies copies of kRandStates Philox states, allocated and seeded on its first
 // sampling call or per-device seed. Copy i is seeded with dev + i*16 + global_seed*127 (global seed
@@ -10,6 +11,7 @@
 // GPU's compute lane, so calls, seeds and state reads stay in issue order.
 #include <cstdlib>
 #include <cstring>
+#include <functional>
 #include <string>
 
 #include "engine.h"
@@ -57,6 +59,21 @@ DevRandom& Generators(int dev) {
   return R;
 }
 
+void RandomNormal(const OpInfo& op, const std::vector<NDArray>& in, std::vector<NDArray>* outputs,
+                  const Params& p) {
+  const char* n = op.name;
+  RejectUnknownKeys(p, {"loc", "scale", "shape", "ctx", "dtype"});
+  KV_CHECK(in.empty()) << n << " takes no inputs";
+  const float loc = GetF(p, "loc", 0.0f);
+  const float scale = GetF(p, "scale", 1.0f);
+  const SampleTarget t = ParseSampleTarget(n, p, *outputs, false);
+  KV_CHECK(scale > 0) << "scale parameter in gaussian has to be positive";
+  NDArray o = OutOr(outputs, 0, t.shape, t.ctx, t.dtype);
+  RandNormalInto(o, loc, scale, true);
+}
+
+}  // namespace
+
 // "gpu(1)", "cpu(0)", "cpu_pinned(0)" (Context::FromString); an empty string is the CPU
 Context ParseCtx(const std::string& s, const char* op) {
   if (s.empty()) return Context::CPU();
@@ -87,9 +104,13 @@ std::vector<int64_t> ParseShape(const std::string& s, const char* op) {
   return out;
 }
 
-// SampleNormalParam's dtype enum, and bfloat16 as an extension; -1 is None
-int ParseDType(const std::string& s, const char* op) {
+int ParseDType(const std::string& s, const char* op, bool integer) {
   if (s == "None") return -1;
+  if (integer) {
+    if (s == "int32") return kInt32;
+    if (s == "int64") return kInt64;
+    KV_FATAL << op << ": Invalid Input: '" << s << "', valid values are: {'None', 'int32', 'int64'}";
+  }
   if (s == "float32") return kFloat32;
   if (s == "float64") return kFloat64;
   if (s == "float16") return kFloat16;
@@ -99,56 +120,64 @@ int ParseDType(const std::string& s, const char* op) {
   return -1;
 }
 
-void RandomNormal(const OpInfo& op, const std::vector<NDArray>& in, std::vector<NDArray>* outputs,
-                  const Params& p) {
-  const char* n = op.name;
-  RejectUnknownKeys(p, {"loc", "scale", "shape", "ctx", "dtype"});
-  KV_CHECK(in.empty()) << n << " takes no inputs";
-  const float loc = GetF(p, "loc", 0.0f);
-  const float scale = GetF(p, "scale", 1.0f);
+SampleTarget ParseSampleTarget(const char* n, const Params& p, const std::vector<NDArray>& outputs,
+                               bool integer) {
   const std::string* shape_s = Find(p, "shape");
   const std::string* dtype_s = Find(p, "dtype");
   const std::string* ctx_s = Find(p, "ctx");
   const bool has_shape = shape_s != nullptr && !ParseShape(*shape_s, n).empty();
-  const std::vector<int64_t> shape = has_shape ? ParseShape(*shape_s, n) : std::vector<int64_t>();
-  int dtype = dtype_s != nullptr ? ParseDType(*dtype_s, n) : -1;
-  Context ctx = ParseCtx(ctx_s != nullptr ? *ctx_s : "", n);
-  if (!outputs->empty()) {
+  SampleTarget t;
+  if (has_shape) t.shape = ParseShape(*shape_s, n);
+  t.dtype = dtype_s != nullptr ? ParseDType(*dtype_s, n, integer) : -1;
+  t.ctx = ParseCtx(ctx_s != nullptr ? *ctx_s : "", n);
+  if (!outputs.empty()) {
     // the output's context, shape and dtype decide; a given shape or dtype must agree with them
-    const NDArray& o = (*outputs)[0];
+    const NDArray& o = outputs[0];
     KV_CHECK(o.stype() == kDefaultStorage) << n << ": out must be a dense array; got " << StypeName(o.stype());
-    KV_CHECK(!has_shape || o.shape() == shape) << n << ": out has the wrong shape";
-    KV_CHECK(dtype == -1 || o.dtype() == dtype) << n << ": out dtype " << DTypeName(o.dtype())
-                                                << " differs from dtype " << DTypeName(dtype);
-    dtype = o.dtype();
-    ctx = o.ctx();
+    KV_CHECK(!has_shape || o.shape() == t.shape) << n << ": out has the wrong shape";
+    KV_CHECK(t.dtype == -1 || o.dtype() == t.dtype) << n << ": out dtype " << DTypeName(o.dtype())
+                                                    << " differs from dtype " << DTypeName(t.dtype);
+    t.shape = o.shape();
+    t.dtype = o.dtype();
+    t.ctx = o.ctx();
   } else {
     KV_CHECK(has_shape) << n << ": shape is required when no out is given";
   }
-  if (dtype == -1) dtype = kFloat32;
-  KV_CHECK(dtype == kFloat32 || dtype == kFloat64 || dtype == kFloat16 || dtype == kBfloat16)
-      << n << ": float16, bfloat16, float32 and float64 outputs only; got " << DTypeName(dtype);
-  KV_CHECK(ctx.dev_type == kGPU) << n << " samples on the GPU only (the reference's CPU generator is a "
-                                 << "different stream)";
-  KV_CHECK(scale > 0) << "scale parameter in gaussian has to be positive";
-  NDArray o = OutOr(outputs, 0, shape, ctx, dtype);
-  RandNormalInto(o, loc, scale, true);
+  if (t.dtype == -1) t.dtype = integer ? kInt32 : kFloat32;
+  CheckSampleDType(n, t.dtype, integer);
+  KV_CHECK(t.ctx.dev_type == kGPU) << n << " samples on the GPU only (the reference's CPU generator is a "
+                                   << "different stream)";
+  return t;
 }
 
-}  // namespace
+void CheckSampleDType(const char* n, int dtype, bool integer) {
+  if (integer) {
+    KV_CHECK(dtype == kInt32 || dtype == kInt64) << n << ": int32 and int64 outputs only; got "
+                                                 << DTypeName(dtype);
+  } else {
+    KV_CHECK(dtype == kFloat32 || dtype == kFloat64 || dtype == kFloat16 || dtype == kBfloat16)
+        << n << ": float16, bfloat16, float32 and float64 outputs only; got " << DTypeName(dtype);
+  }
+}
 
-void RandNormalInto(const NDArray& out, float loc, float scale, bool staged) {
-  KV_CHECK(out.on_gpu() && out.stype() == kDefaultStorage) << "_random_normal: out must be a dense GPU array";
+void SampleInto(const NDArray& out, const char* launch_name,
+                const std::function<void(void* states, cudaStream_t stream)>& launch) {
+  KV_CHECK(out.on_gpu() && out.stype() == kDefaultStorage) << launch_name << ": out must be a dense GPU array";
   const int dev = out.dev();
   DevRandom& R = Generators(dev);
   const size_t i = ++R.curr_ptr % kRandCopies;
   LaneOp lop(dev);
   lop.Write(&R.var[i]).Write(out);
-  const uint64_t size = out.Size();
-  LaunchRandNormal(out.dtype(), R.states[i], size > 0 ? out.data() : nullptr, size, loc, scale, staged,
-                   lop.stream());
-  if (size > 0) Engine::Get()->CountLaunch("_random_normal", size * DTypeSize(out.dtype()));
+  launch(R.states[i], lop.stream());
+  if (out.Size() > 0) Engine::Get()->CountLaunch(launch_name, out.Size() * DTypeSize(out.dtype()));
   lop.Issue();
+}
+
+void RandNormalInto(const NDArray& out, float loc, float scale, bool staged) {
+  const uint64_t size = out.Size();
+  SampleInto(out, "_random_normal", [&](void* states, cudaStream_t stream) {
+    LaunchRandNormal(out.dtype(), states, size > 0 ? out.data() : nullptr, size, loc, scale, staged, stream);
+  });
 }
 
 void RandomSeed(uint32_t seed) {

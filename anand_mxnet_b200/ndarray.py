@@ -733,12 +733,16 @@ contrib = _Contrib()
 
 
 class _Random(object):
-    """mx.nd.random: the samplers of mx.random (random.py)"""
+    """mx.nd.random: the samplers of mx.random (random.py), and the _like operators, which the
+    reference's op module places here"""
+    _NAMES = ('uniform', 'normal', 'randn', 'exponential', 'gamma', 'randint',
+              'uniform_like', 'normal_like', 'exponential_like', 'gamma_like')
 
-    @property
-    def normal(self):
-        from .random import normal as _normal
-        return _normal
+    def __getattr__(self, name):
+        if name not in _Random._NAMES:
+            raise AttributeError("mx.nd.random has no attribute '%s'" % name)
+        from . import random as _random
+        return getattr(_random, name)
 
 
 random = _Random()
