@@ -95,11 +95,12 @@ void LaunchDenseFused(const DenseLaunch& p, cudaStream_t stream);
 // float16, bfloat16, float32, float64, int32 and int64. `scalar` is the operator's double; the kernel
 // converts it once to the array's dtype, as the reference's DType(alpha) / static_cast<DType>(value).
 // kEwClip takes its float bounds a_min, a_max as `scalar`, `scalar2` and compares them with each
-// element as the reference's clip kernel does. kEwDiv and kEwDivScalar divide floating types only.
+// element as the reference's clip kernel does. kEwDiv, kEwDivScalar and kEwRDivScalar (scalar / a)
+// divide floating types only.
 // b_row > 0 makes `b` one value per row of b_row elements (b[i / b_row]); 0: b has n elements.
 enum EwOp : int {
   kEwCopy = 0, kEwAdd, kEwSub, kEwMul, kEwAddScalar, kEwMulScalar, kEwFill, kEwSqrt,
-  kEwDiv, kEwMax, kEwDivScalar, kEwAbs, kEwClip, kEwSquare
+  kEwDiv, kEwMax, kEwDivScalar, kEwAbs, kEwClip, kEwSquare, kEwRDivScalar
 };
 bool ElementwiseDTypeOk(int dtype);
 void LaunchElementwise(int op, int dtype, void* out, const void* a, const void* b, double scalar,
@@ -320,13 +321,22 @@ void LaunchRandNormal(int dtype, void* states, void* out, uint64_t n, float loc,
 //   kRandGamma        Marsaglia-Tsang, shape a, scale b
 //   kRandInt          lo + rand_int64() % (hi - lo), hi > lo    (int32, int64)
 // The first three write float16, bfloat16, float32 or float64. No launch when n == 0.
-enum RandDist { kRandUniform, kRandExponential, kRandGamma, kRandInt };
+// (kRandNormal is the multi-sample normal; the scalar normal is LaunchRandNormal.)
+enum RandDist { kRandUniform, kRandExponential, kRandGamma, kRandInt, kRandNormal };
 struct RandParams {
   float a = 0.0f, b = 0.0f;
   int64_t lo = 0, hi = 0;
 };
 void LaunchRandSample(int dist, int dtype, void* states, void* out, uint64_t n, const RandParams& p,
                       cudaStream_t stream);
+// The multi-sample samplers of multisample_op.h in the same mapping and staged store: element i of
+// out[0, n) draws kRandUniform (low a, high b), kRandNormal (mu a, sigma b), kRandExponential (lam
+// a; b unused) or kRandGamma (alpha a, beta b) with parameters a[i / nBatch], b[i / nBatch], nBatch
+// = n / nparm. ptype (the parameter arrays) and otype (out): float16, float32 or float64. A gamma
+// element that exhausts its attempt budget is NaN. out may be a (the same bytes) when nparm == n.
+// No launch when n == 0.
+void LaunchRandSampleParams(int dist, int ptype, int otype, void* states, const void* a, const void* b,
+                            uint64_t nparm, void* out, uint64_t n, cudaStream_t stream);
 
 // ---- single-tensor optimizer operators of the callback route (update_kernels.cu) ----
 // nag_mom_update, mp_nag_mom_update, signsgd_update, signum_update, rmsprop_update,

@@ -124,6 +124,7 @@ __global__ void ew_kernel(int op, T* out, const T* a, const T* b, double scalar,
       case kEwAbs: r = Abs(x); break;
       case kEwClip: r = Clip(x, static_cast<float>(scalar), static_cast<float>(scalar2)); break;
       case kEwSquare: r = Square(x); break;
+      case kEwRDivScalar: r = Div(Widen(s), x); break;  // mshadow_op::rdiv
       default: r = Sqrt(x); break;  // kEwSqrt
     }
     out[i] = Narrow<T>(r);

@@ -91,7 +91,7 @@ const OpInfo* FindOp(const std::string& name) {
     auto* m = new std::unordered_map<std::string, const OpInfo*>();
     for (const std::vector<OpInfo>* family :
          {&kCoreOps, &kMultiTensorOps, &kUpdateOps, &kArithOps, &kReduceOps, &kSumOps, &kRandomOps,
-          &kSampleOps}) {
+          &kSampleOps, &kSampleParamOps}) {
       for (const OpInfo& op : *family) {
         KV_CHECK(m->emplace(op.name, &op).second) << "operator " << op.name << " is declared twice";
       }

@@ -31,9 +31,9 @@ struct OpInfo {
 enum OpFlags { kOpMom = 1, kOpMp = 2, kOpMulti = 4, kOpPreloaded = 8 };
 
 // each family's operators: ops.cc, multi_ops.cc, update_ops.cc, arith_ops.cc, reduce_ops.cc, sum_ops.cc,
-// random_ops.cc, sample_ops.cc
+// random_ops.cc, sample_ops.cc, sample_param_ops.cc
 extern const std::vector<OpInfo> kCoreOps, kMultiTensorOps, kUpdateOps, kArithOps, kReduceOps, kSumOps,
-    kRandomOps, kSampleOps;
+    kRandomOps, kSampleOps, kSampleParamOps;
 
 // nullptr when the operator is not registered
 const OpInfo* FindOp(const std::string& name);

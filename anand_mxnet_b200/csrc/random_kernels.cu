@@ -70,10 +70,11 @@ struct Draw<__nv_bfloat16> {
 
 // The staged store of thread t's run: len elements from draw(&st) (len == 0: t draws nothing), through
 // the warp's shared tile, to out[t*step, t*step + len). vec: out and step allow 16-B vectors. Every
-// lane of the warp calls it.
+// lane of the warp calls it. draw is called once per element in run order (it may keep a cursor),
+// and every element's draw happens before the warp stores that element.
 template <typename T, typename DrawFn>
 __device__ __forceinline__ void DrawRunStaged(curandStatePhilox4_32_10_t* st, T* __restrict__ out, uint64_t step,
-                                              uint64_t len, uint32_t t, uint32_t vec, const DrawFn& draw) {
+                                              uint64_t len, uint32_t t, uint32_t vec, DrawFn&& draw) {
   constexpr int kRun = 128 / sizeof(T);         // elements a lane draws per round
   constexpr int kPerVec = 16 / sizeof(T);
   constexpr int kPad = sizeof(T) >= 4 ? 1 : 4 / sizeof(T);  // tile rows 4 B apart in banks
@@ -182,51 +183,104 @@ struct Out<__nv_bfloat16> {
   static __device__ __forceinline__ __nv_bfloat16 Of(X x) { return __float2bfloat16_rn(static_cast<float>(x)); }
 };
 
-// SampleUniformKernel: OType(lower + (upper - lower) * uniform()), lower and upper float
-template <typename T>
-struct UniformDraw {
-  float lower, upper;
-  __device__ __forceinline__ T operator()(curandStatePhilox4_32_10_t* s) const {
-    const Gen<T> u = Uniform01<Gen<T>>(s);
-    return Out<T>::Of(lower + (upper - lower) * u);
-  }
+// mshadow's half_t as a parameter type (half.h): every operator with a half_t operand rounds
+// float(a) OP float(b) to half, and a comparison compares the two floats. The multi-sample kernels
+// do their parameter arithmetic in it, as the reference's do with IType half_t.
+struct HalfT {
+  __half h;
+  HalfT() = default;
+  __device__ __forceinline__ HalfT(float f) : h(__float2half_rn(f)) {}
+  __device__ __forceinline__ operator float() const { return __half2float(h); }
 };
+static_assert(sizeof(HalfT) == 2, "a float16 parameter array is read as HalfT");
+#define B200KV_HALF_OP(R, OP)                                                                           \
+  __device__ __forceinline__ R operator OP(HalfT a, HalfT b) { return R(float(a) OP float(b)); }           \
+  template <typename X>                                                                                    \
+  __device__ __forceinline__ R operator OP(HalfT a, X b) { return R(float(a) OP float(b)); }               \
+  template <typename X>                                                                                    \
+  __device__ __forceinline__ R operator OP(X a, HalfT b) { return R(float(a) OP float(b)); }
+B200KV_HALF_OP(HalfT, +)
+B200KV_HALF_OP(HalfT, -)
+B200KV_HALF_OP(HalfT, *)
+B200KV_HALF_OP(HalfT, /)
+B200KV_HALF_OP(bool, <)
+B200KV_HALF_OP(bool, >)
+#undef B200KV_HALF_OP
 
-// SampleExponentialKernel: OType(-log(1.0 - uniform()) / lambda), in double
-template <typename T>
-struct ExponentialDraw {
-  float lambda;
-  __device__ __forceinline__ T operator()(curandStatePhilox4_32_10_t* s) const {
-    const Gen<T> u = Uniform01<Gen<T>>(s);
-    return Out<T>::Of(-log(1.0 - u) / lambda);
-  }
-};
+// The draws of sampler.h with parameters of type P (float for the scalar samplers; IType for the
+// multi-sample ones), written as the reference writes them so that the mixed float / double / half_t
+// arithmetic and its contraction are the same.
+
+// SampleUniformKernel: OType(lower + (upper - lower) * uniform())
+template <typename T, typename P>
+__device__ __forceinline__ T UniformOf(curandStatePhilox4_32_10_t* s, P lower, P upper) {
+  const Gen<T> u = Uniform01<Gen<T>>(s);
+  return Out<T>::Of(lower + (upper - lower) * u);
+}
+
+// SampleNormalKernel: OType(normal() * std + mean)
+template <typename T, typename P>
+__device__ __forceinline__ T NormalOf(curandStatePhilox4_32_10_t* s, P mean, P std) {
+  return Out<T>::Of(Normal01<Gen<T>>(s) * std + mean);
+}
+
+// SampleExponentialKernel: OType(-log(1.0 - uniform()) / lambda)
+template <typename T, typename P>
+__device__ __forceinline__ T ExponentialOf(curandStatePhilox4_32_10_t* s, P lambda) {
+  const Gen<T> u = Uniform01<Gen<T>>(s);
+  return Out<T>::Of(-log(1.0 - u) / lambda);
+}
 
 // SampleGamma in FType = Gen<T>: Marsaglia-Tsang, one normal and one uniform per attempt that gets
 // past Z > -k, and one more uniform for alpha < 1. The literals are double, as in the reference, so
 // d, k and c are rounded from double and the acceptance test is evaluated in double.
+//
+// The reference loops until an attempt is accepted, which never happens when d is NaN, <= 0 or +inf
+// (alpha NaN, +-inf or <= -2/3). Here an element gets kGammaAttempts attempts; one that exhausts
+// them is NaN, without alpha < 1's last uniform, and the thread goes on to its next element. For
+// alpha > 0, d >= 2/3 and an attempt fails with probability below about 0.05, so a valid element
+// exhausts the budget with probability near 1e-80 (DESIGN.md §8).
+constexpr int kGammaAttempts = 64;
+template <typename T, typename P>
+__device__ __forceinline__ T GammaOf(curandStatePhilox4_32_10_t* s, P alpha, P beta) {
+  using F = Gen<T>;
+  const F d = alpha < 1 ? alpha + 2.0 / 3.0 : alpha - 1.0 / 3.0;
+  const F k = sqrt(9.0 * d);
+  const F c = 1.0 / k;
+  F sample;
+  int attempt = 0;
+  for (; attempt < kGammaAttempts; ++attempt) {
+    const F z = Normal01<F>(s);
+    if (z > -k) {
+      const F x = 1.0 + c * z;
+      const F v = x * x * x;
+      if (log(1.0 - Uniform01<F>(s)) < 0.5 * z * z + d * (1.0 - v + log(v))) {
+        sample = d * v * beta;
+        break;
+      }
+    }
+  }
+  if (attempt == kGammaAttempts) return Out<T>::Of(F(NAN));
+  return Out<T>::Of(alpha < 1 ? sample * pow(Uniform01<F>(s), F(1.0 / alpha)) : sample);
+}
+
+// the scalar samplers' draws (sample_op.h: float parameters)
+template <typename T>
+struct UniformDraw {
+  float lower, upper;
+  __device__ __forceinline__ T operator()(curandStatePhilox4_32_10_t* s) const { return UniformOf<T>(s, lower, upper); }
+};
+
+template <typename T>
+struct ExponentialDraw {
+  float lambda;
+  __device__ __forceinline__ T operator()(curandStatePhilox4_32_10_t* s) const { return ExponentialOf<T>(s, lambda); }
+};
+
 template <typename T>
 struct GammaDraw {
   float alpha, beta;
-  __device__ __forceinline__ T operator()(curandStatePhilox4_32_10_t* s) const {
-    using F = Gen<T>;
-    const F d = alpha < 1 ? alpha + 2.0 / 3.0 : alpha - 1.0 / 3.0;
-    const F k = sqrt(9.0 * d);
-    const F c = 1.0 / k;
-    F sample;
-    while (true) {
-      const F z = Normal01<F>(s);
-      if (z > -k) {
-        const F x = 1.0 + c * z;
-        const F v = x * x * x;
-        if (log(1.0 - Uniform01<F>(s)) < 0.5 * z * z + d * (1.0 - v + log(v))) {
-          sample = d * v * beta;
-          break;
-        }
-      }
-    }
-    return Out<T>::Of(alpha < 1 ? sample * pow(Uniform01<F>(s), F(1.0 / alpha)) : sample);
-  }
+  __device__ __forceinline__ T operator()(curandStatePhilox4_32_10_t* s) const { return GammaOf<T>(s, alpha, beta); }
 };
 
 // SampleRandIntKernel with int64 bounds: OType(lower + rand_int64() % (upper - lower)), where
@@ -268,6 +322,73 @@ __global__ void __launch_bounds__(kDrawThreads)
   if (len > 0) states[t] = st;
 }
 
+// ---- the multi-sample kernels of multisample_op.h: sampler.h's kernels with nParm > 1, element i
+// drawing with parameters i / nBatch, nBatch = 1 + (N - 1) / nParm. P is the parameter arrays' type
+// (HalfT for float16), T the output's.
+
+// A thread's parameter cursor: a and b point at the parameters of the next element it draws, and
+// left elements remain in their batch. Set once per thread from the run's first element and advanced
+// per draw, so the hot loop divides nothing. Each draw reads its parameters before the element is
+// stored (DrawRunStaged), so out may be a parameter array itself (nBatch 1).
+template <int kDist, typename P, typename T>
+struct ParamDraw {
+  const P* a;
+  const P* b;
+  uint64_t nbatch, left;
+  __device__ __forceinline__ T operator()(curandStatePhilox4_32_10_t* s) {
+    const P x = *a;
+    const P y = kDist == kRandExponential ? x : *b;
+    if (--left == 0) {
+      left = nbatch;
+      ++a;
+      ++b;
+    }
+    if constexpr (kDist == kRandUniform) return UniformOf<T>(s, x, y);
+    else if constexpr (kDist == kRandNormal) return NormalOf<T>(s, x, y);
+    else if constexpr (kDist == kRandExponential) return ExponentialOf<T>(s, x);
+    else return GammaOf<T>(s, x, y);
+  }
+};
+
+// x / d and x % d for x < 2^52 from the host's inv = 1.0 / d: the double product is within one of
+// the quotient, which one correction step settles (no 64-bit division routine, so no stack frame)
+__device__ __forceinline__ void DivModBatch(uint64_t x, uint64_t d, double inv, uint64_t* q, uint64_t* r) {
+  uint64_t qq = static_cast<uint64_t>(static_cast<double>(x) * inv);
+  int64_t rr = static_cast<int64_t>(x - qq * d);
+  if (rr < 0) {
+    --qq;
+    rr += static_cast<int64_t>(d);
+  } else if (rr >= static_cast<int64_t>(d)) {
+    ++qq;
+    rr -= static_cast<int64_t>(d);
+  }
+  *q = qq;
+  *r = static_cast<uint64_t>(rr);
+}
+
+// min blocks 1: without it ptxas caps some instantiations near 40-64 registers and spills; a full
+// launch is 512 CTAs, about 4 per SM, so the registers cost no occupancy the launch could use
+template <int kDist, typename P, typename T>
+__global__ void __launch_bounds__(kDrawThreads, 1)
+    param_draw_kernel(curandStatePhilox4_32_10_t* states, T* out, uint64_t n, uint64_t step, uint32_t nthread,
+                      const P* a, const P* b, uint64_t nbatch, double inv_nbatch, uint32_t vec) {
+  const uint32_t t = blockIdx.x * kDrawThreads + threadIdx.x;
+  const uint64_t start = static_cast<uint64_t>(t) * step;
+  const uint64_t len = t < nthread && start < n ? (n - start < step ? n - start : step) : 0;
+  curandStatePhilox4_32_10_t st;
+  ParamDraw<kDist, P, T> draw{a, b, nbatch, 0};
+  if (len > 0) {
+    st = states[t];
+    uint64_t p, rem;
+    DivModBatch(start, nbatch, inv_nbatch, &p, &rem);
+    draw.a += p;
+    draw.b += p;
+    draw.left = nbatch - rem;
+  }
+  DrawRunStaged(&st, out, step, len, t, vec, draw);
+  if (len > 0) states[t] = st;
+}
+
 // LaunchRNG's nthread and step for n > 0 elements, the grid, and whether 16-B stores apply
 struct DrawShape {
   uint64_t nthread, step;
@@ -300,6 +421,39 @@ void LaunchFloatSample(int dist, void* states, void* out, uint64_t n, const Rand
     case kRandExponential: LaunchSample<T>(states, out, n, ExponentialDraw<T>{p.a}, st); break;
     case kRandGamma: LaunchSample<T>(states, out, n, GammaDraw<T>{p.a, p.b}, st); break;
     default: KV_FATAL << "random sampler " << dist << " has no floating-point form";
+  }
+}
+
+template <int kDist, typename P, typename T>
+void LaunchParam(void* states, const void* a, const void* b, uint64_t nparm, void* out, uint64_t n,
+                 cudaStream_t st) {
+  const DrawShape d = ShapeFor<T>(out, n);
+  const uint64_t nbatch = 1 + (n - 1) / nparm;
+  param_draw_kernel<kDist, P, T><<<d.blocks, kDrawThreads, 0, st>>>(
+      static_cast<curandStatePhilox4_32_10_t*>(states), static_cast<T*>(out), n, d.step,
+      static_cast<uint32_t>(d.nthread), static_cast<const P*>(a), static_cast<const P*>(b), nbatch,
+      1.0 / static_cast<double>(nbatch), d.vec);
+}
+
+template <int kDist, typename P>
+void LaunchParamOut(int otype, void* states, const void* a, const void* b, uint64_t nparm, void* out, uint64_t n,
+                    cudaStream_t st) {
+  switch (otype) {
+    case kFloat16: LaunchParam<kDist, P, __half>(states, a, b, nparm, out, n, st); break;
+    case kFloat32: LaunchParam<kDist, P, float>(states, a, b, nparm, out, n, st); break;
+    case kFloat64: LaunchParam<kDist, P, double>(states, a, b, nparm, out, n, st); break;
+    default: KV_FATAL << "multi-sample: unsupported output dtype " << DTypeName(otype);
+  }
+}
+
+template <int kDist>
+void LaunchParamDist(int ptype, int otype, void* states, const void* a, const void* b, uint64_t nparm, void* out,
+                     uint64_t n, cudaStream_t st) {
+  switch (ptype) {
+    case kFloat16: LaunchParamOut<kDist, HalfT>(otype, states, a, b, nparm, out, n, st); break;
+    case kFloat32: LaunchParamOut<kDist, float>(otype, states, a, b, nparm, out, n, st); break;
+    case kFloat64: LaunchParamOut<kDist, double>(otype, states, a, b, nparm, out, n, st); break;
+    default: KV_FATAL << "multi-sample: unsupported parameter dtype " << DTypeName(ptype);
   }
 }
 
@@ -358,6 +512,21 @@ void LaunchRandSample(int dist, int dtype, void* states, void* out, uint64_t n, 
       case kFloat64: LaunchFloatSample<double>(dist, states, out, n, p, st); break;
       default: KV_FATAL << "random sampler: unsupported dtype " << DTypeName(dtype);
     }
+  }
+  KV_CUDA(cudaGetLastError());
+}
+
+void LaunchRandSampleParams(int dist, int ptype, int otype, void* states, const void* a, const void* b,
+                            uint64_t nparm, void* out, uint64_t n, cudaStream_t st) {
+  if (n == 0) return;
+  KV_CHECK(nparm > 0 && n % nparm == 0) << "multi-sample: " << n << " outputs for " << nparm << " parameters";
+  KV_CHECK(n < (uint64_t{1} << 52)) << "multi-sample: " << n << " outputs is past the kernel's index range";
+  switch (dist) {
+    case kRandUniform: LaunchParamDist<kRandUniform>(ptype, otype, states, a, b, nparm, out, n, st); break;
+    case kRandNormal: LaunchParamDist<kRandNormal>(ptype, otype, states, a, b, nparm, out, n, st); break;
+    case kRandExponential: LaunchParamDist<kRandExponential>(ptype, otype, states, a, a, nparm, out, n, st); break;
+    case kRandGamma: LaunchParamDist<kRandGamma>(ptype, otype, states, a, b, nparm, out, n, st); break;
+    default: KV_FATAL << "multi-sample: no sampler " << dist;
   }
   KV_CUDA(cudaGetLastError());
 }

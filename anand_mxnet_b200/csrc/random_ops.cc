@@ -161,12 +161,14 @@ void CheckSampleDType(const char* n, int dtype, bool integer) {
 }
 
 void SampleInto(const NDArray& out, const char* launch_name,
-                const std::function<void(void* states, cudaStream_t stream)>& launch) {
+                const std::function<void(void* states, cudaStream_t stream)>& launch,
+                const std::vector<NDArray>& reads) {
   KV_CHECK(out.on_gpu() && out.stype() == kDefaultStorage) << launch_name << ": out must be a dense GPU array";
   const int dev = out.dev();
   DevRandom& R = Generators(dev);
   const size_t i = ++R.curr_ptr % kRandCopies;
   LaneOp lop(dev);
+  for (const NDArray& a : reads) lop.Read(a);
   lop.Write(&R.var[i]).Write(out);
   launch(R.states[i], lop.stream());
   if (out.Size() > 0) Engine::Get()->CountLaunch(launch_name, out.Size() * DTypeSize(out.dtype()));

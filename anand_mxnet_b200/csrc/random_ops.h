@@ -19,9 +19,11 @@ void RandomSeed(uint32_t seed);
 void RandomSeedContext(uint32_t seed, Context ctx);
 // One sampling call into a dense GPU array: the device's next generator copy (++curr_ptr % 4) and
 // out are declared as writes of one operation on the GPU's compute lane, and launch(states, stream)
-// issues the draw from that copy. launch_name and out's bytes go to Engine::CountLaunch.
+// issues the draw from that copy. launch_name and out's bytes go to Engine::CountLaunch. reads: the
+// arrays the draw reads (the multi-sample operators' parameters; out may be one of them).
 void SampleInto(const NDArray& out, const char* launch_name,
-                const std::function<void(void* states, cudaStream_t stream)>& launch);
+                const std::function<void(void* states, cudaStream_t stream)>& launch,
+                const std::vector<NDArray>& reads = {});
 // normal(loc, scale) into a dense GPU array from the device's next generator copy; staged = false
 // selects the reference's per-thread store order (measurement only)
 void RandNormalInto(const NDArray& out, float loc, float scale, bool staged);

@@ -7,6 +7,7 @@
 // dmlc::stof; randint's int64 bounds: an integer literal) and checked as sample_op.h checks them,
 // before any generator is created or advanced.
 #include <cerrno>
+#include <cmath>
 #include <cstdlib>
 #include <string>
 
@@ -65,6 +66,8 @@ RandParams DistParams(int dist, const char* n, const Params& p) {
       r.b = GetF(p, "beta", 1.0f);
       KV_CHECK(r.a > 0) << "alpha parameter in gamma distribution has to be positive";
       KV_CHECK(r.b > 0) << "beta parameter in gamma distribution has to be positive";
+      // this library's own check: the reference's draw never ends for alpha = +inf
+      KV_CHECK(std::isfinite(r.a)) << n << ": alpha must be finite (the gamma draw does not end for alpha = inf)";
       break;
     case kRandInt: {
       r.lo = RequiredInt64(p, "low", n);

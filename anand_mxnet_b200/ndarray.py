@@ -250,6 +250,12 @@ class NDArray(object):
     def __itruediv__(self, other):
         return self._binary(other, 'broadcast_div', '_div_scalar', out=self)
 
+    def __rtruediv__(self, other):
+        """scalar / array (_rdiv_scalar), floating dtypes only"""
+        return _invoke('_rdiv_scalar', [self], scalar=float(other))
+
+    __rdiv__ = __rtruediv__
+
     def __getitem__(self, key):
         """a[b:e] on the first axis: a view sharing memory (MXNDArraySlice, ndarray.py:_slice)"""
         if isinstance(key, int):
@@ -536,6 +542,13 @@ def _op(name):
 
 
 sgd_update = _op('sgd_update')
+# the multi-sample operators under the reference's generated names: sample_uniform(low, high,
+# shape=(), dtype=None, out=None) and likewise sample_normal(mu, sigma), sample_gamma(alpha, beta),
+# sample_exponential(lam)
+sample_uniform = _op('sample_uniform')
+sample_normal = _op('sample_normal')
+sample_gamma = _op('sample_gamma')
+sample_exponential = _op('sample_exponential')
 sgd_mom_update = _op('sgd_mom_update')
 mp_sgd_update = _op('mp_sgd_update')
 mp_sgd_mom_update = _op('mp_sgd_mom_update')
